@@ -3,7 +3,8 @@
 PKG    = fluent-bit_b200
 CSRC   = $(PKG)/csrc
 NVCC  ?= nvcc
-NVFLAGS = -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC
+ARCH   = -gencode arch=compute_90a,code=sm_90a
+NVFLAGS = $(ARCH) -lineinfo -O3 -std=c++17 -Xcompiler -fPIC
 CFLAGS = -O2 -g -fPIC -Wall -Wno-unused-function
 
 all: product hostsim oracle
@@ -24,7 +25,7 @@ $(CSRC)/runtime.o: $(CSRC)/runtime.c $(HDRS)
 $(CSRC)/rx_compile.o: $(CSRC)/rx_compile.c $(HDRS)
 	gcc $(CFLAGS) -c $(CSRC)/rx_compile.c -o $@
 $(PKG)/libflbgpu.so: $(CSRC)/kernels.o $(CSRC)/kernels_ml.o $(CSRC)/kernels_tojson.o $(CSRC)/kernels_lines.o $(CSRC)/runtime.o $(CSRC)/rx_compile.o
-	$(NVCC) -shared -o $@ $(CSRC)/kernels.o $(CSRC)/kernels_ml.o $(CSRC)/kernels_tojson.o $(CSRC)/kernels_lines.o $(CSRC)/runtime.o $(CSRC)/rx_compile.o -lcudart -lpthread -ldl
+	$(NVCC) $(ARCH) -shared -o $@ $(CSRC)/kernels.o $(CSRC)/kernels_ml.o $(CSRC)/kernels_tojson.o $(CSRC)/kernels_lines.o $(CSRC)/runtime.o $(CSRC)/rx_compile.o -lcudart -lpthread -ldl
 
 hostsim: tests/hostsim/libhostsim.so
 tests/hostsim/libhostsim.so: tests/hostsim/hostsim.cpp $(CSRC)/runtime.c $(CSRC)/rx_compile.c $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h)

@@ -3,6 +3,7 @@
 
   python bench.py --gpus N --steps K --warmup W            (ours; torchrun for N>1)
   python bench.py --impl reference --gpus N --steps K --warmup W
+  python bench.py ... --dump-outputs DIR                  (also writes the last timed step's result, see dump_outputs)
 
 Primary workload (config.workload): BASELINE.json configs[1] -- 10 M JSON lines through filter_parser(json) +
 filter_grep + filter_modify, 10 M events per GPU per step (weak scaling).  A step is one pass of the chain over
@@ -388,7 +389,7 @@ class ClockSampler(threading.Thread):
 
     def run(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), "--query-gpu=" + q,
                                           "--format=csv,noheader,nounits", "-lms", "200"],
@@ -405,8 +406,9 @@ class ClockSampler(threading.Thread):
         mx = [float(r[1]) for r in self.rows if len(r) > 1 and r[1].replace(".", "").isdigit()]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for i, n in enumerate(names) if any(len(r) > 3 + i and r[3 + i].lower().startswith("active") for r in self.rows)]
+        lim = [float(r[7]) for r in self.rows if len(r) > 7 and r[7].replace(".", "").isdigit()]
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": reasons,
-                "samples": len(sm)}
+                "power_limit_w": lim[-1] if lim else None, "samples": len(sm)}
 
 
 _libc = C.CDLL(None)
@@ -480,20 +482,30 @@ class Workload:
     def device_setup(self):
         L, ctx = self.L, self.ctx
         self.d_in = L.flbgpu_dev_alloc(ctx.h, self.nbytes + 64)
-        self.out_cap = self.segs[0][1] + self.segs[0][1] // 2 + 4096
-        self.d_out = L.flbgpu_dev_alloc(ctx.h, self.out_cap)
+        self.out_cap = (self.segs[0][1] + self.segs[0][1] // 2 + 4096 + 4095) & ~4095
+        self.d_out = L.flbgpu_dev_alloc(ctx.h, self.out_cap * len(self.segs))     # one result range per call of a step
         assert self.d_in and self.d_out, "device allocation failed"
         L.flbgpu_dev_upload(ctx.h, self.d_in, self.h_page, self.nbytes)
 
     def step_device(self):
-        total = 0
-        for off, n in self.segs:
-            r = self.L.flbgpu_chain_do_device(self.chain.h, self.d_in + off, n, self.d_out, self.out_cap, C.byref(self.osz))
+        self.out_sizes = []
+        for k, (off, n) in enumerate(self.segs):
+            r = self.L.flbgpu_chain_do_device(self.chain.h, self.d_in + off, n, self.d_out + k * self.out_cap, self.out_cap, C.byref(self.osz))
             if r != self.pkg.FILTER_MODIFIED:
                 raise RuntimeError("chain_do_device -> %d: %s" % (r, self.ctx.err()))
-            total += self.osz.value
-        self.out_total = total
+            self.out_sizes.append(self.osz.value)
+        self.out_total = sum(self.out_sizes)
         self.exchange()
+
+    def device_result(self):
+        """the chunk the last step_device() returned: its calls' results, in order"""
+        buf = C.create_string_buffer(max(1, self.out_total))
+        at = 0
+        for k, n in enumerate(self.out_sizes):
+            if n and self.L.flbgpu_dev_download(self.ctx.h, C.byref(buf, at), self.d_out + k * self.out_cap, n) != 0:
+                raise RuntimeError("dev_download: %s" % self.ctx.err())
+            at += n
+        return buf.raw[:self.out_total]
 
     # ---- host buffers through the C ABI
     def call(self, chain, ptr, n):
@@ -537,6 +549,34 @@ class Workload:
         return out
 
 
+DUMP_WINDOW = 4096          # bytes per sampled window of the result
+DUMP_WINDOWS = 256
+DUMP_BLOCK = 65536          # bytes per checksum block
+
+
+def dump_outputs(directory, result, out_sizes):
+    """What the timed device-resident step returned, as float arrays (at most a few MB for any batch size):
+      result_sizes.npy ....... float64, bytes returned by each call of the step
+      result_checksums.npy ... float64 [blocks, 2], per 64 KiB block of the result: sum of the bytes, and sum of
+                               byte * (position in the block + 1) -- both exact in float64; every byte counts
+      result_sample.npy ...... float32, the byte values of 256 windows of 4 KiB at fixed offsets (seeded), or the whole
+                               result when it is smaller than that"""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    b = np.frombuffer(result, dtype=np.uint8)
+    np.save(os.path.join(directory, "result_sizes.npy"), np.asarray(out_sizes, dtype=np.float64))
+    pad = np.zeros(-len(b) % DUMP_BLOCK, dtype=np.uint8)
+    blocks = np.concatenate([b, pad]).reshape(-1, DUMP_BLOCK).astype(np.float64)
+    weights = np.arange(1, DUMP_BLOCK + 1, dtype=np.float64)
+    np.save(os.path.join(directory, "result_checksums.npy"), np.stack([blocks.sum(axis=1), blocks @ weights], axis=1))
+    if len(b) <= DUMP_WINDOW * DUMP_WINDOWS:
+        sample = b
+    else:
+        starts = np.sort(np.random.default_rng(0xF1B1).choice(len(b) - DUMP_WINDOW, DUMP_WINDOWS, replace=False))
+        sample = np.concatenate([b[s:s + DUMP_WINDOW] for s in starts])
+    np.save(os.path.join(directory, "result_sample.npy"), sample.astype(np.float32))
+
+
 def timed(fn, barrier):
     barrier()
     t0 = time.perf_counter()
@@ -545,11 +585,11 @@ def timed(fn, barrier):
     return time.perf_counter() - t0
 
 
-def measure(args, wl, L, ctx, torch, dist, rank, world, local, full=True):
-    """value / e2e / kernel times of one workload on this rank's GPU"""
+def measure(args, wl, L, ctx, torch, dist, rank, world, local, full=True, dump=None):
+    """value / e2e / kernel times of one workload on this rank's GPU; dump: directory for the last timed step's result"""
     w = Workload(args, wl, L, ctx, rank, world)
     n_lines, nbytes = w.n_lines, w.nbytes
-    steps = args.steps if wl not in ("c0",) else max(args.steps, 20)
+    steps = args.steps
 
     def barrier():
         torch.cuda.synchronize()
@@ -586,6 +626,8 @@ def measure(args, wl, L, ctx, torch, dist, rank, world, local, full=True):
     barrier()
     dev_ms = allmax(ev0.elapsed_time(ev1))
     clocks = sampler.stop()
+    if dump:
+        dump_outputs(dump, w.device_result(), w.out_sizes)
     st1 = w.chain.stats()
     launches = int(st1.kernel_launches - st0.kernel_launches)
     out_bytes = w.out_total
@@ -700,7 +742,7 @@ def measure_tojson(args, L, ctx, torch, world):
         return n.value
     for _ in range(max(3, args.warmup)):
         text_bytes = call()
-    reps = max(10, args.steps * 4)
+    reps = args.steps
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     kms = [0.0, 0.0, 0.0]
@@ -746,7 +788,7 @@ def measure_textpath(args, L, ctx, torch, world):
         return n, len(js)
     for _ in range(max(3, args.warmup)):
         n, nbytes = call()
-    reps = max(5, args.steps * 2)
+    reps = args.steps
     torch.cuda.synchronize()
     t0 = time.perf_counter()
     for _ in range(reps):
@@ -780,7 +822,8 @@ def run_ours(args):
         dist.broadcast_object_list(box, src=0)
         ctx.comm_init(world, rank, box[0])
     WL = args.workload
-    m = measure(args, WL, L, ctx, torch, dist, rank, world, local, full=True)
+    m = measure(args, WL, L, ctx, torch, dist, rank, world, local, full=True,
+                dump=(args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, "rank%d" % rank)) if args.dump_outputs else None)
     others = {}
     if not args.primary_only:
         for o in ("apache", "c0", "nginx", "l2m", "ml"):
@@ -850,13 +893,8 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    traffic = None
-    try:
-        per_event = json.load(open(os.path.join(ROOT, "profiles", "traffic.json"))).get("k_chain_eval_dram_bytes_per_event_" + WL)
-        traffic = per_event * m["n_lines"] if per_event else None      # ncu dram read+write of the evaluation launches of one step
-    except Exception:
-        pass
+    peak = float(peaks.get("hbm_gbs", 3350.0))           # H100 SXM data sheet: 3.35 TB/s of HBM3
+    props = torch.cuda.get_device_properties(local)
 
     def roof(mm):
         eval_ms = mm["kms"][1]
@@ -898,7 +936,7 @@ def run_ours(args):
         "scaling": "weak", "vs_baseline": None, "dtype": "u8", "data": "synthetic",
         "config": {"workload": WORKLOADS[WL]["name"], "events_per_gpu_per_step": m["n_lines"], "distinct_lines": BASE_LINES},
         "config_detail": {"input_bytes_per_gpu": m["nbytes"], "output_bytes_per_gpu": m["out_bytes"],
-                          "l2": "input (%.0f MB) and output larger than the 126 MB L2" % (m["nbytes"] / 1e6),
+                          "l2": "input %.0f MB, L2 of the %s %.0f MB" % (m["nbytes"] / 1e6, props.name, props.L2_cache_size / 1e6),
                           "parallelism": ("record shards; one NCCL all-reduce of the metric table per step" if WL == "l2m" else "record shards, no data-path collective"),
                           "e2e_input": "pageable malloc()ed memory", "e2e_host_malloc": "glibc, untouched"},
         "e2e": {"value": m["e2e"], "unit": "lines/s", "h2d_bytes_per_step": m["nbytes"], "d2h_bytes_per_step": m["out_bytes"],
@@ -909,11 +947,12 @@ def run_ours(args):
         "kernel_ms_per_step": {"index": m["kms"][0], "evaluate": eval_ms, "emit": m["kms"][2],
                                "note": "CUDA-event pairs per launch group; index runs on its own priority stream concurrently with evaluate, so the groups are not additive"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": (achieved / peak) if achieved else None, "traffic": traffic,
+                     "frac": (achieved / peak) if achieved else None,
                      "kernel": "k_chain_eval (evaluation pass)", "algorithmic_bytes_per_launch": alg_bytes,
-                     "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback 6650 GB/s"},
+                     "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet, 3350 GB/s"},
         "cpu_baseline": cpu,
         "clocks": m["clocks"],
+        "device": props.name,
     }
     if "apache" in others:
         line["north_star"] = side(others.pop("apache"), "apache")
@@ -939,6 +978,7 @@ def main():
     ap.add_argument("--l2m-total", type=int, default=100_000_000, help="records of configs[3] over all GPUs")
     ap.add_argument("--workload", default="json", choices=list(WORKLOADS), help="primary workload (the others are reported beside it)")
     ap.add_argument("--primary-only", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the result of the last timed device-resident step as .npy files")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

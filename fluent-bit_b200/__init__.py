@@ -1,6 +1,6 @@
 """fluent-bit_b200 -- Python mirror (ctypes) of the libflbgpu C ABI (include/flbgpu.h).
 
-The product is the C-ABI library `libflbgpu.so` next to this file (CUDA, sm_100a).  This
+The product is the C-ABI library `libflbgpu.so` next to this file (CUDA, sm_90a).  This
 module only binds it for tests and bench.py; it contains no compute and no fallback:
 importing works without a GPU, but `Context()` raises when the library is missing or no
 CUDA device is usable.

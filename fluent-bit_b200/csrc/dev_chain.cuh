@@ -298,7 +298,7 @@ FLB_HD const uint8_t *rec_frame(const uint8_t *p, const uint8_t *end, int *kind)
     if (q >= end || mp_token(q, end, &t) != 0) return 0;
     if (t.type == MPT_UINT) sec = (int64_t) t.u;
     else if (t.type == MPT_INT) { if ((int64_t) t.u < 0) return 0; sec = (int64_t) t.u; }
-    else if (t.type == MPT_F64) { union { uint64_t u; double d; } cv; cv.u = t.u; sec = (int64_t) cv.d; }
+    else if (t.type == MPT_F64) { union { uint64_t u; double d; } cv; cv.u = t.u; sec = mp_d2i64(cv.d); }   /* whether the decoder steps over it: as x86-64 converts */
     else if (t.type == MPT_EXT) {
         if (t.ext_type != 0 || t.len != 8 || (size_t) (end - q) < t.hdr + 8u) return 0;
         sec = (int64_t) (int32_t) mp_be32(q + t.hdr);

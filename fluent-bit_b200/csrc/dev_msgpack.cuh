@@ -36,6 +36,14 @@ FLB_HD uint32_t mp_be32(const uint8_t *p)
 }
 FLB_HD uint64_t mp_be64(const uint8_t *p) { return ((uint64_t) mp_be32(p) << 32) | mp_be32(p + 4); }
 
+/* (int64_t) of a double as the reference's x86-64 build converts it (cvttsd2si): out of range and NaN give INT64_MIN, where
+ * the device's conversion would saturate / give 0 */
+FLB_HD int64_t mp_d2i64(double d)
+{
+    if (!(d >= -9223372036854775808.0 && d < 9223372036854775808.0)) return (int64_t) 0x8000000000000000ull;
+    return (int64_t) d;
+}
+
 /* token classes */
 enum { MPT_NIL = 0, MPT_BOOL, MPT_UINT, MPT_INT, MPT_F32, MPT_F64, MPT_STR, MPT_BIN, MPT_ARRAY, MPT_MAP,
        MPT_EXT, MPT_INVALID };

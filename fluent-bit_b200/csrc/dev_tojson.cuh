@@ -313,14 +313,6 @@ FLB_HD uint32_t tj_datetime(int64_t sec, uint64_t usec, int iso, uint8_t *o)
 }
 
 
-/* (int64_t) of a double as the reference's x86-64 build converts it (cvttsd2si): out of range and NaN give INT64_MIN, where
- * the device's conversion would saturate / give 0 */
-FLB_HD int64_t tj_d2i64(double d)
-{
-    if (!(d >= -9223372036854775808.0 && d < 9223372036854775808.0)) return (int64_t) 0x8000000000000000ull;
-    return (int64_t) d;
-}
-
 /* the event as one msgpack map in its scratch slice (flb_pack.c:1380-1497); returns its length */
 FLB_HDN uint32_t tj_pack_event(const struct tj_env *e, uint32_t i, uint8_t *b)
 {
@@ -335,8 +327,8 @@ FLB_HDN uint32_t tj_pack_event(const struct tj_env *e, uint32_t i, uint8_t *b)
     else if (t.type == MPT_F64) {
         union { uint64_t u; double d; } cv;
         cv.u = t.u;
-        sec = tj_d2i64(cv.d);
-        nsec = tj_d2i64((cv.d - (double) sec) * 1000000000.0);
+        sec = mp_d2i64(cv.d);
+        nsec = mp_d2i64((cv.d - (double) sec) * 1000000000.0);
     }
     else { sec = (int64_t) (int32_t) mp_be32(q + t.hdr); nsec = (int64_t) (int32_t) mp_be32(q + t.hdr + 4); }
     q += t.hdr + (t.type == MPT_EXT ? t.len : 0);
@@ -529,7 +521,7 @@ FLB_HDN uint32_t tj_event(const struct tj_env *e, uint32_t i, uint8_t *o)
             mp_token(q, p + e->len[i], &t);
             if (t.type == MPT_EXT) sec = (long long) (int32_t) mp_be32(q + t.hdr);
             else if (t.type == MPT_INT || t.type == MPT_UINT) sec = (long long) (int32_t) (uint32_t) t.u;
-            else if (t.type == MPT_F64) { union { uint64_t u; double d; } cv; cv.u = t.u; sec = (long long) (int32_t) (uint32_t) tj_d2i64(cv.d); }
+            else if (t.type == MPT_F64) { union { uint64_t u; double d; } cv; cv.u = t.u; sec = (long long) (int32_t) (uint32_t) mp_d2i64(cv.d); }
             if (sec == -1 || sec == -2) {
 #ifdef __CUDA_ARCH__
                 const unsigned long long at = atomicAdd(e->n_marks, 1ull);

@@ -1,6 +1,6 @@
 /* flbgpu_internal.h -- seam between the host runtime (C) and the device back end.
  *
- * The product library links runtime.c + kernels.cu (CUDA, sm_100a) and nothing
+ * The product library links runtime.c + kernels.cu (CUDA, sm_90a) and nothing
  * else: there is no CPU implementation of bk_* in libflbgpu.so, so every entry
  * point fails loudly when no CUDA device is present.  tests/hostsim provides a
  * second implementation of the same functions for CPU-only CI of the host logic

@@ -1,4 +1,4 @@
-/* kernels.cu -- sm_100a kernels and the CUDA implementation of the bk_* seam.
+/* kernels.cu -- sm_90a kernels and the CUDA implementation of the bk_* seam.
  *
  *   k_index<FILL> ..... K1 record index: every 0x92 byte is a record candidate; a
  *                       candidate is kept when a complete, well-formed log event
@@ -46,9 +46,8 @@ static std::atomic<unsigned long long> g_launches;
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { \
     snprintf(g_err, sizeof(g_err), "%s: %s", #call, cudaGetErrorString(e_)); return -1; } } while (0)
 
-/* 4 resident blocks per SM (64 registers per lane): measured best on B200 -- the interpreter is bound
- * by instruction fetch and load latency, which more resident warps hide better than fewer spills do
- * (profiles/r01_variants.txt) */
+/* 4 resident blocks per SM (64 registers per lane): the interpreter is bound by instruction fetch and load
+ * latency, which more resident warps hide better than fewer spills do */
 #ifndef BK_EVAL_MIN_BLOCKS
 #define BK_EVAL_MIN_BLOCKS 4
 #endif
@@ -385,10 +384,10 @@ __device__ __forceinline__ uint32_t bm_mask4(uint32_t w)
 /* PH: CH_PH_ALL = the whole chain in one launch.  Split form (chains `parser, then other filters`): a CH_PH_HEAD launch
  * decodes and parses and leaves the field lists in the capture cache, a CH_PH_TAIL launch runs the other filters from there.
  * Each half has roughly half the interpreter's code, which is what the single launch is bound by (instruction cache misses,
- * profiles/r02_ncu_eval_json.txt). */
+ * the interpreter's hot code does not fit an SM's instruction cache). */
 template <int PH>
 __global__ void __launch_bounds__(1024, 1) k_chain_eval_t(const __grid_constant__ k_chain_params p)       /* 64 registers per lane; block size chosen at launch.
-                                                                                                             (5 or 6 resident blocks of 256 lanes with 48 / 40 registers: slower, profiles/r02_variants.txt) */
+                                                                                                             (5 or 6 resident blocks of 256 lanes with 48 / 40 registers were slower) */
 {
     extern __shared__ __align__(16) uint8_t dsm[];
     const uint32_t n_rec = p.n_dev ? *p.n_dev : p.n_rec;
@@ -570,7 +569,7 @@ __global__ void __launch_bounds__(BK_REC_BLOCK) k_surv_fill(const uint32_t *__re
 /* One lane encodes one surviving record.  The survivors of a warp are consecutive in the result (the list is in
  * record order and the offsets are a running sum), so the warp first encodes its 32 records into a slice of shared
  * memory laid out like the result, then copies the whole range out with coalesced 16-byte stores: the result leaves
- * the SM in full sectors instead of byte-sized partial writes (profiles/: DRAM write bytes per result byte 3.7 -> ~1).
+ * the SM in full sectors instead of byte-sized partial writes (about one DRAM write byte per result byte).
  * A warp whose range does not fit its slice writes directly, as before. */
 #define EMIT_BLOCK 128u
 #define EMIT_STAGE 8192u          /* bytes of result per warp that can be staged (+16 of alignment slack) */
@@ -776,9 +775,10 @@ struct bk_q {
     uint8_t *h_sin, *h_sout; size_t cap_sin, cap_sout;    /* small form: pinned staging for the chunk and its result */
     cudaEvent_t ev_small;
     int json_bm;                           /* FLBGPU_JSON_BM=1: two-stage JSON tokenizer (stage-1 bitmap + bit-scan walker + deferral).
-                                              Off by default: measured 20 % slower than the byte scanner on configs[1]
-                                              (profiles/r02_variants.txt) -- the walker's lanes diverge on the value type */
+                                              Off by default in the single launch: slower there than the byte scanner
+                                              -- the walker's lanes diverge on the value type */
     int eval_block;                        /* FLBGPU_EVAL_BLOCK: threads per evaluation block */
+    int n_sm;                              /* multiprocessors of the device: the grid of the grid-stride launches */
     uint8_t *d_tag; size_t cap_tag;        /* rewrite_tag: the tag of the call; the re-tagged stream before it goes to the host */
     uint8_t *d_eout; size_t cap_eout;
     unsigned long long *d_stage; size_t cap_stage;   /* index: what the counting pass validated, one row per tile */
@@ -875,7 +875,7 @@ static void ev_end_on(bk_q *q, int k, cudaStream_t st)
 
 extern "C" {
 
-const char *bk_name(void) { return "cuda-sm_100a"; }
+const char *bk_name(void) { return "cuda-sm_90a"; }
 const char *bk_last_error(void) { return g_err; }
 uint64_t bk_launch_count(void) { return g_launches.load(); }
 /* for the other translation units of the back end (kernels_ml.cu): the launch counter and the calling thread's error text */
@@ -972,6 +972,7 @@ static int q_setup(bk_q *q)
     int lo = 0, hi = 0;
     CK(cudaSetDevice(q->device));
     if (func_attrs_once()) return -1;
+    CK(cudaDeviceGetAttribute(&q->n_sm, cudaDevAttrMultiProcessorCount, q->device));
     CK(cudaStreamCreateWithFlags(&q->stream, cudaStreamNonBlocking));
     /* the index kernels of the next slice are short and the host waits for their result: let their
      * blocks go ahead of the thousands of queued evaluation blocks of the previous slice */
@@ -1024,7 +1025,7 @@ bk_q *bk_q_new(int device)
     if (!mem) { snprintf(g_err, sizeof(g_err), "out of memory"); return 0; }
     q = new (mem) bk_q;
     q->device = device;
-    q->xf_slots = 16;                 /* measured best on the bench box: 16 x 8 MiB (profiles/r01_variants.txt) */
+    q->xf_slots = 16;                 /* 16 x 8 MiB; FLBGPU_XF_SLOTS / FLBGPU_XF_MB */
     q->xf_slice = (size_t) 8 << 20;
     if (cudaSetDevice(device) != cudaSuccess) { snprintf(g_err, sizeof(g_err), "cudaSetDevice(%d) failed", device); q->~bk_q(); free(q); return 0; }
     bind_near_device(device);
@@ -1383,13 +1384,13 @@ int bk_flags_clear(bk_q *q, uint32_t *d_flags)
 
 /* The slice of input the next evaluation reads is touched once: mark it as streaming in L2 (access
  * policy window of the stream) so that it does not evict the lanes' local-memory lines (field lists,
- * regex stacks), which are re-used by every block.  Measured without effect (profiles/r01_variants.txt), so it
+ * regex stacks), which are re-used by every block.  It had no measurable effect, so it
  * is opt-in: FLBGPU_L2_WINDOW=1. */
 int bk_hint_streaming(bk_q *q, const void *base, size_t bytes)
 {
     static int max_win = -1, enabled = -1;
     cudaStreamAttrValue v;
-    if (enabled < 0) { const char *e = getenv("FLBGPU_L2_WINDOW"); enabled = (e && e[0] == '1'); }   /* off: no measurable effect on B200 */
+    if (enabled < 0) { const char *e = getenv("FLBGPU_L2_WINDOW"); enabled = (e && e[0] == '1'); }   /* off by default: see above */
     if (!enabled) return 0;
     use(q);
     if (max_win < 0) {
@@ -1448,7 +1449,7 @@ int bk_chain_eval(bk_q *q, const struct bk_chain_args *a, uint32_t r0, uint32_t 
          * evaluated BESIDE the tail launch -- the two touch different records */
         CK(cudaEventRecord(q->d_ev[0], q->stream));
         CK(cudaStreamWaitEvent(q->dstream, q->d_ev[0], 0));
-        k_chain_eval_deferred<<<148 * 4, BK_REC_BLOCK, 0, q->dstream>>>(p);
+        k_chain_eval_deferred<<<q->n_sm * 4, BK_REC_BLOCK, 0, q->dstream>>>(p);
         CK(cudaEventRecord(q->d_ev[1], q->dstream));
         k_chain_eval_t<CH_PH_TAIL><<<grid, q->eval_block, 0, q->stream>>>(p);
         CK(cudaStreamWaitEvent(q->stream, q->d_ev[1], 0));
@@ -1456,7 +1457,7 @@ int bk_chain_eval(bk_q *q, const struct bk_chain_args *a, uint32_t r0, uint32_t 
     }
     else {
         k_chain_eval<<<(r1 - r0 + q->eval_block - 1) / q->eval_block, q->eval_block, (size_t) p.bm_words * 4 * (q->eval_block / 32), q->stream>>>(p);
-        if (p.defer_list) { k_chain_eval_deferred<<<148 * 4, BK_REC_BLOCK, 0, q->stream>>>(p); g_launches += 1; }
+        if (p.defer_list) { k_chain_eval_deferred<<<q->n_sm * 4, BK_REC_BLOCK, 0, q->stream>>>(p); g_launches += 1; }
     }
     if (p.env.l2m.hash) {
         k_chain_skipped<<<(r1 - r0 + BK_REC_BLOCK - 1) / BK_REC_BLOCK, BK_REC_BLOCK, 0, q->stream>>>(p);
@@ -1692,7 +1693,7 @@ int bk_small_run(bk_q *q, const struct bk_chain_args *a, const void *h_in, uint8
     }
     else
         k_chain_eval<<<nb_cap, BK_REC_BLOCK, (size_t) p.bm_words * 4 * (BK_REC_BLOCK / 32), st>>>(p);
-    if (p.defer_list) { k_chain_eval_deferred<<<148, BK_REC_BLOCK, 0, st>>>(p); g_launches += 1; }
+    if (p.defer_list) { k_chain_eval_deferred<<<q->n_sm, BK_REC_BLOCK, 0, st>>>(p); g_launches += 1; }
     if (p.env.l2m.hash) {
         k_chain_skipped<<<nb_cap, BK_REC_BLOCK, 0, st>>>(p); g_launches += 1;
         if (p.env.l2m.pending) { k_l2m_fixup<<<1, 1024, 0, st>>>(p); k_l2m_fixup_done<<<1, 1, 0, st>>>(p); g_launches += 2; }

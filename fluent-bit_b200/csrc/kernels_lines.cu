@@ -1,4 +1,4 @@
-/* kernels_lines.cu -- raw text to log events on sm_100a (in_tail's line loop): the launches behind bk_ln_*.
+/* kernels_lines.cu -- raw text to log events on sm_90a (in_tail's line loop): the launches behind bk_ln_*.
  *
  *   k_ln_count ... one lane per tile of LN_TILE bytes: the line feeds of the tile (neighbouring lanes read neighbouring tiles)
  *   k_ln_fill .... the same lanes again: positions of the line feeds at the tile's offset (block offsets from the scan, the rest

@@ -1,4 +1,4 @@
-/* kernels_ml.cu -- filter_multiline on sm_100a: the launches behind bk_ml_plan / bk_ml_sizes / bk_ml_emit.
+/* kernels_ml.cu -- filter_multiline on sm_90a: the launches behind bk_ml_plan / bk_ml_sizes / bk_ml_emit.
  *
  * All the work is in dev_ml.cuh (the same functions the CPU emulation of the tests loops over); a kernel here gives every
  * piece its thread:

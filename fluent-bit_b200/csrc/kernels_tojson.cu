@@ -1,4 +1,4 @@
-/* kernels_tojson.cu -- a chunk of log events as JSON text on sm_100a: the launches behind bk_tj_sizes / bk_tj_emit.
+/* kernels_tojson.cu -- a chunk of log events as JSON text on sm_90a: the launches behind bk_tj_sizes / bk_tj_emit.
  *
  * One lane per event, two passes over dev_tojson.cuh's tj_event(): the sizing pass packs the event as one msgpack map into its
  * scratch slice (what the reference converts from) and measures the text; after the scan over the sizes the emission pass

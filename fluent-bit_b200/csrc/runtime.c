@@ -1490,8 +1490,8 @@ int flbgpu_chain_init(flbgpu_chain *c)
         for (k2 = 0; k2 < last_parser; k2++) if (c->f[k2]->kind == FLBGPU_F_LOG_TO_METRICS) c->defer_ok = 0;
         /* `parser, then filters that are not parsers`: the evaluation runs as two launches (kernels.cu: k_chain_eval_t) */
         {
-            /* Measured (profiles/r02_variants.txt): -31 % evaluation time when the parser is the JSON transcoder (the largest piece
-             * of code), +5 % when it is a regex parser -- so by default only the former.  FLBGPU_EVAL_SPLIT=1 / 0 forces it. */
+            /* The split pays when the parser is the JSON transcoder (the largest piece of code) and costs when it is a regex
+             * parser (two launches re-load what one keeps) -- so by default only the former.  FLBGPU_EVAL_SPLIT=1 / 0 forces it. */
             const char *e = getenv("FLBGPU_EVAL_SPLIT");
             const int want = e ? e[0] != '0' : (c->f[0]->needs_scratch & 1);
             c->split = c->nf >= 2 && last_parser == 0 && want;
@@ -1647,7 +1647,7 @@ static int ensure_rec_cap(flbgpu_chain *c, size_t need, size_t keep)
 static size_t slice_bytes(void)
 {
     const char *e = getenv("FLBGPU_SLICE_MB");
-    size_t mb = e ? (size_t) atol(e) : 128;       /* measured best end to end on B200 (profiles/r01_variants.txt) */
+    size_t mb = e ? (size_t) atol(e) : 128;       /* not re-tuned on H100: FLBGPU_SLICE_MB */
     if (mb < 1) mb = 1;
     if (mb > 2048) mb = 2048;
     return mb << 20;

@@ -43,7 +43,9 @@ int flbgpu_lines_to_events(flbgpu_ctx *ctx, const char *text, size_t bytes, cons
 #define LN_GROW(ptr, cap, n_, type) do { if ((cap) < (size_t) (n_)) { size_t nc_ = (size_t) (n_) + (size_t) (n_) / 4 + 64; \
         bk_free(c->q, ptr); (ptr) = (type *) bk_alloc(c->q, nc_ * sizeof(type)); if (!(ptr)) { (cap) = 0; LN_FAIL(); } (cap) = nc_; } } while (0)
     LN_GROW(c->d_in, c->cap_in, bytes + 64, uint8_t);
-    if (bk_upload_start(c->q, c->d_in, (const uint8_t *) text, bytes) || bk_upload_wait_index(c->q, bytes)) LN_FAIL();
+    /* on the compute stream, where the line kernels run: the staged upload (bk_upload_start) orders only the index stream, so
+     * the counting pass could read text that has not arrived and the filling pass write more line feeds than were counted */
+    if (bk_h2d(c->q, c->d_in, text, bytes)) LN_FAIL();
     e.text = c->d_in;
     /* work memory: the strings, the counts per tile; the line arrays once the number of lines is known */
     need = 1024 + 16 + sizeof(uint32_t) * (size_t) e.n_tiles + 64;

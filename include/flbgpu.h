@@ -1,4 +1,4 @@
-/* flbgpu.h -- C ABI of libflbgpu.so: Fluent Bit's parse->filter hot path on B200.
+/* flbgpu.h -- C ABI of libflbgpu.so: Fluent Bit's parse->filter hot path on H100.
  *
  * Plain C, plain pointers and sizes.  Each entry point names the reference
  * interface it stands in for (paths relative to the fluent-bit source tree, v5.0.2).

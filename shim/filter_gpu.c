@@ -311,7 +311,7 @@ static int cb_exit_rewrite_tag(void *data, struct flb_config *config)
 
 extern struct flb_filter_plugin filter_rewrite_tag_plugin;
 struct flb_filter_plugin filter_gpu_rewrite_tag_plugin = {
-    .name = "gpu_rewrite_tag", .description = "B200: rewrite_tag on the GPU (libflbgpu)",
+    .name = "gpu_rewrite_tag", .description = "H100: rewrite_tag on the GPU (libflbgpu)",
     .cb_init = cb_init_rewrite_tag, .cb_filter = cb_filter_rewrite_tag, .cb_exit = cb_exit_rewrite_tag, .flags = 0 };
 
 /* the metric table of a gpu_log_to_metrics instance in cmetrics' text form (what the stock plugin appends to its
@@ -328,7 +328,7 @@ extern struct flb_filter_plugin filter_parser_plugin, filter_grep_plugin, filter
     static int cb_init_##sym(struct flb_filter_instance *ins, struct flb_config *config, void *data)         \
     { (void) data; return gpu_init(ins, config, short_name); }                                              \
     struct flb_filter_plugin filter_gpu_##sym##_plugin = {                                                   \
-        .name = gpu_name, .description = "B200: " short_name " on the GPU (libflbgpu)",                       \
+        .name = gpu_name, .description = "H100: " short_name " on the GPU (libflbgpu)",                       \
         .cb_init = cb_init_##sym, .cb_filter = cb_gpu_filter, .cb_exit = cb_gpu_exit, .flags = 0 };
 
 GPU_PLUGIN(parser, "parser", "gpu_parser", filter_parser_plugin)

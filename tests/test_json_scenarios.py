@@ -1,8 +1,9 @@
 """The reference's JSON fixtures through filter_parser(json): tests/internal/data/pack/* (the packed
 string its pack test expects must come out) and benchmarks/utf8_surrogate_bench_10k.ndjson (two
-lines of each of its 11 kinds as golden vectors; all 10 000 live when the reference tree is here).
-tests/golden/json_scenarios.json is made by tests/golden/make_json_scenarios.py."""
+lines of each of its 11 kinds as golden vectors; all 10 000, stored as tests/golden/utf8_surrogate_bench_10k.ndjson.xz,
+against the reference's results).  tests/golden/json_scenarios.json is made by tests/golden/make_json_scenarios.py."""
 import json
+import lzma
 import os
 
 import pytest
@@ -13,7 +14,7 @@ pkg = util.pkg
 SCENARIOS = json.load(open(os.path.join(util.ROOT, "tests", "golden", "json_scenarios.json")))
 KW = dict(name="js", format="json")
 PROPS = [("Key_Name", "log"), ("Parser", "js")]
-NDJSON = "/root/reference/benchmarks/utf8_surrogate_bench_10k.ndjson"
+NDJSON = os.path.join(util.ROOT, "tests", "golden", "utf8_surrogate_bench_10k.ndjson.xz")
 
 
 def run(lib):
@@ -41,9 +42,8 @@ def test_json_scenarios_gpu(gpu_lib):
     run(gpu_lib)
 
 
-@pytest.mark.skipif(not os.path.exists(NDJSON), reason="the reference tree is not on this machine")
 def test_whole_surrogate_corpus_live(sim_lib, ref_available):
-    lines = [l.rstrip(b"\n") for l in open(NDJSON, "rb")]
+    lines = [l.rstrip(b"\n") for l in lzma.open(NDJSON, "rb")]
     assert len(lines) == 10000
     chunk = util.chunk_from_lines(lines)
     ctx, ref = pkg.Context(0, lib=sim_lib), util.Ref()

@@ -17,12 +17,7 @@ TS = re.compile(r"^\S+Z ", re.M)
 
 
 def ref_text(ref, f):
-    ref.L.flbref_l2m_cmt_text.restype = C.c_void_p
-    ref.L.flbref_l2m_cmt_text.argtypes = [C.c_void_p]
-    p = ref.L.flbref_l2m_cmt_text(f)
-    t = C.string_at(p).decode(errors="replace")
-    ref.L.flbref_cfree(C.c_void_p(p))
-    return TS.sub("", t)
+    return TS.sub("", ref.l2m_text(f))
 
 
 def run_case(lib, parsers, filters, chunk, k, calls=2):

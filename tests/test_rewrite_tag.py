@@ -11,14 +11,6 @@ pkg = util.pkg
 S = util.mp_str
 
 
-def grouped(pairs):
-    """the state the reference's per-record in_emitter_add_record() calls leave in the emitter: one buffer per tag"""
-    d = {}
-    for t, b in pairs:
-        d.setdefault(t, []).append(b)
-    return [(t, b"".join(v), len(v)) for t, v in d.items()]
-
-
 def run(lib, rules, chunk, tag="app.web.x", parsers=(), before=(), after=(), fail_after=-1):
     ref = util.Ref()
     ref.emit_reset(fail_after)
@@ -30,7 +22,7 @@ def run(lib, rules, chunk, tag="app.web.x", parsers=(), before=(), after=(), fai
         ref.filter(p, props)
         fs.append(ctx.filter(p, props))
     want = ref.chain_do(chunk, tag=tag)
-    want_emit = grouped(ref.emitted())
+    want_emit = ref.emitted_grouped()
     got = ctx.chain(fs).do(chunk, tag=tag)
     got_emit = fs[len(before)].emitted()
     return got, got_emit, want, want_emit
@@ -115,7 +107,7 @@ def _in_chains(lib):
     ours = {}
     for t, d, n in fa.emitted() + fb.emitted():
         ours[t] = (ours.get(t, (b"", 0))[0] + d, ours.get(t, (b"", 0))[1] + n)
-    assert [(t, d, n) for t, (d, n) in ours.items()] == grouped(ref.emitted())
+    assert [(t, d, n) for t, (d, n) in ours.items()] == ref.emitted_grouped()
 
 
 def _odd_chunks(lib):

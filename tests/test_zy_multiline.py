@@ -279,7 +279,7 @@ def _reference_runtime_unbuffered(lib):
     Compared with the reference's plugin record for record, the eight timestamp bytes apart; then the same six lines in ONE chunk
     (and with real timestamps): one message."""
     props = [("multiline.key_content", "log"), ("multiline.parser", "go"), ("buffer", "off"), ("debug_flush", "off")]
-    ref = util.Ref()
+    ref = util.Ref(keep_whole=True)
     rf = ref.filter("multiline", props)
     ctx = pkg.Context(0, lib=lib)
     ch = ctx.chain([ctx.filter("multiline", props)])
@@ -312,7 +312,7 @@ def _edge_chunks(lib):
     props = [("multiline.parser", "java"), ("multiline.key_content", "log"), ("buffer", "off")]
     one = util.event(5, 0, [(b"log", S(b"x"))])
     for c in (mk, mk * 3, mk + one + mk, b"\xc1garbage", one + b"\xc1\xc1", util.event(0, 0, [(b"other", b"\x01")])):
-        ref = util.Ref()
+        ref = util.Ref(keep_whole=True)
         rf = ref.filter("multiline", props)
         ctx = pkg.Context(0, lib=lib)
         got, want = ctx.chain([ctx.filter("multiline", props)]).do(c), ref.filter_cb(rf, c)

@@ -1,7 +1,13 @@
-"""Shared test helpers: reference harness binding (oracle/_ref), event encoding,
+"""Shared test helpers: reference harness binding (oracle/_ref) with its stored transcript, event encoding,
 synthetic line generators (SURVEY.md section 8d)."""
+import atexit
+import base64
 import ctypes as C
+import functools
+import gzip
+import hashlib
 import importlib
+import json
 import os
 import random
 import struct
@@ -10,18 +16,180 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 REF_SO = os.path.join(ROOT, "oracle", "_ref", "libflbref.so")
 SHIM_SO = os.path.join(ROOT, "oracle", "_ref", "flb-filter_gpu.so")
 HOSTSIM_SO = os.environ.get("FLBGPU_HOSTSIM_SO") or os.path.join(ROOT, "tests", "hostsim", "libhostsim.so")   # override: a sanitizer build
+TRANSCRIPT = os.path.join(ROOT, "tests", "golden", "ref_transcript.json.gz")
+RECORD = os.environ.get("FLBGPU_REF_RECORD") == "1"
 
 pkg = importlib.import_module("fluent-bit_b200")
 
 
 def have_ref():
+    """the reference build itself is here (oracle/_ref, made by build() where the reference tree is)"""
     return os.path.exists(REF_SO)
 
 
-class Ref:
-    """The UNMODIFIED reference code (oracle/_ref/libflbref.so)."""
+# ------------------------------------------------------------ reference transcript
+# What the reference returned to every test that compares with it, in call order per test, so that those tests run
+# where the reference build is absent.  FLBGPU_REF_RECORD=1 with oracle/_ref built rewrites the transcript of the tests
+# that ran.  Text and outputs up to INLINE bytes are stored whole; longer outputs as their length and a SHA-256 prefix
+# (RefDigest), which compares equal to the bytes it was taken of -- unless the Ref was made with
+# keep_whole=True, for a test that compares parts of the outputs.  Entries: "s<text>", "b<base64>", "h<digest><length>",
+# ["T" or "L", entries...] for a tuple or list, "H" for an object the reference made, {"raise": message}, or a number.
+INLINE = 8
+DIGEST_HEX = 8
 
+
+class RefDigest:
+    """A stored reference output too long to keep whole: equal to the bytes it was taken of."""
+
+    def __init__(self, digest, n):
+        self.digest, self.n = digest, n
+
+    @staticmethod
+    def of(b):
+        return hashlib.sha256(b).hexdigest()[:DIGEST_HEX]
+
+    def __eq__(self, other):
+        if isinstance(other, RefDigest):
+            return (self.digest, self.n) == (other.digest, other.n)
+        if isinstance(other, (bytes, bytearray)):
+            return len(other) == self.n and self.of(bytes(other)) == self.digest
+        return NotImplemented
+
+    def __ne__(self, other):
+        r = self.__eq__(other)
+        return r if r is NotImplemented else not r
+
+    __hash__ = None
+
+    def __len__(self):
+        return self.n
+
+    def __repr__(self):
+        return "<reference output: %d bytes, sha256 %s...>" % (self.n, self.digest)
+
+
+class RefHandle:
+    """a parser / filter / multiline parser the reference made, in a replayed transcript"""
+
+
+def _enc(v, whole=False):
+    if v is None or isinstance(v, (bool, int, float)):
+        return v
+    if isinstance(v, str):
+        return "s" + v
+    if isinstance(v, bytes):
+        return "b" + base64.b64encode(v).decode() if whole or len(v) <= INLINE else "h%s%d" % (RefDigest.of(v), len(v))
+    if isinstance(v, (tuple, list)):
+        return ["T" if isinstance(v, tuple) else "L"] + [_enc(x, whole) for x in v]
+    raise TypeError("cannot store %r" % type(v))
+
+
+def _dec(v):
+    if isinstance(v, list):
+        items = [_dec(x) for x in v[1:]]
+        return tuple(items) if v[0] == "T" else items
+    if not isinstance(v, str):
+        return v
+    if v[0] == "s":
+        return v[1:]
+    if v[0] == "b":
+        return base64.b64decode(v[1:])
+    return RefDigest(v[1:1 + DIGEST_HEX], int(v[1 + DIGEST_HEX:]))
+
+
+class _Transcript:
     def __init__(self):
+        self.data = {}
+        if os.path.exists(TRANSCRIPT):
+            with gzip.open(TRANSCRIPT, "rt") as f:
+                self.data = json.load(f)
+        self.fresh = {}
+        self.cur, self.seq = None, 0
+        if RECORD:
+            atexit.register(self.save)
+
+    @staticmethod
+    def test_id():
+        t = os.environ.get("PYTEST_CURRENT_TEST")
+        return t.rsplit(" (", 1)[0] if t else "<outside a test>"
+
+    def _next(self):
+        t = self.test_id()
+        if t != self.cur:
+            self.cur, self.seq = t, 0
+        self.seq += 1
+        return t, self.seq - 1
+
+    def has_current_test(self):
+        return self.test_id() in self.data
+
+    def record(self, entry):
+        t, i = self._next()
+        rows = self.fresh.setdefault(t, [])
+        assert len(rows) == i
+        rows.append(entry)
+
+    def replay(self):
+        t, i = self._next()
+        rows = self.data.get(t)
+        if rows is None or i >= len(rows):
+            raise LookupError("no stored reference result for call %d of %s: rebuild oracle/_ref and record again "
+                              "(FLBGPU_REF_RECORD=1)" % (i, t))
+        return rows[i]
+
+    def save(self):
+        if not self.fresh:
+            return
+        self.data.update(self.fresh)
+        with open(TRANSCRIPT, "wb") as f:          # mtime 0: the same transcript makes the same file
+            with gzip.GzipFile(fileobj=f, mode="wb", mtime=0) as z:
+                z.write(json.dumps(self.data, sort_keys=True, separators=(",", ":")).encode())
+
+
+TRANSCRIPT_DATA = _Transcript()
+
+
+def have_ref_results():
+    """the reference build is here (while recording, the running test gets an entry even if it makes no call), or its
+    stored results for the running test are"""
+    if have_ref():
+        if RECORD:
+            TRANSCRIPT_DATA.fresh.setdefault(TRANSCRIPT_DATA.test_id(), [])
+        return True
+    return TRANSCRIPT_DATA.has_current_test()
+
+
+def _recorded(handle=False):
+    """a Ref method whose result (or RuntimeError) goes to the transcript, or comes from it without the reference build"""
+    def deco(fn):
+        @functools.wraps(fn)
+        def w(self, *a, **k):
+            if self.L is None:
+                e = TRANSCRIPT_DATA.replay()
+                if isinstance(e, dict) and "raise" in e:
+                    raise RuntimeError(e["raise"])
+                return RefHandle() if handle else _dec(e)
+            try:
+                r = fn(self, *a, **k)
+            except RuntimeError as ex:
+                if RECORD:
+                    TRANSCRIPT_DATA.record({"raise": str(ex)})
+                raise
+            if RECORD:
+                TRANSCRIPT_DATA.record("H" if handle else _enc(r, self.keep_whole))
+            return r
+        return w
+    return deco
+
+
+class Ref:
+    """The UNMODIFIED reference code (oracle/_ref/libflbref.so), or its stored transcript where that is not built."""
+
+    def __init__(self, keep_whole=False):
+        self.keep_whole = keep_whole
+        if not have_ref():
+            self.L = None
+            return
         L = C.CDLL(REF_SO)
         vp, cp, sz = C.c_void_p, C.c_char_p, C.c_size_t
         L.flbref_config_create.restype = vp
@@ -58,11 +226,14 @@ class Ref:
     def load_gpu_plugins(self, gpu_lib_path):
         """register the five filter_gpu_*_plugin structs of the shim (oracle/_ref/flb-filter_gpu.so), bound to the
         given implementation of the C ABI (libflbgpu.so, or the CPU emulation in the not-gpu tests)"""
+        if self.L is None:
+            raise RuntimeError("the gpu_* plugins are hosted by the reference build (oracle/_ref), which is absent")
         os.environ["FLBGPU_SHIM_LIB"] = gpu_lib_path
         for name in ("parser", "grep", "modify", "record_modifier", "log_to_metrics", "rewrite_tag", "multiline"):
             if self.L.flbref_plugin_load(self.cfg, SHIM_SO.encode(), ("filter_gpu_%s_plugin" % name).encode()) != 0:
                 raise RuntimeError("cannot load the gpu_%s plugin from %s" % (name, SHIM_SO))
 
+    @_recorded()
     def pack_json_state(self, js):
         """flb_pack_json_state() on a fresh state: (ret, msgpack bytes or None, last_byte, tokens_count)"""
         out, n, last, cnt = C.c_void_p(), C.c_int(), C.c_int(), C.c_int()
@@ -75,10 +246,24 @@ class Ref:
 
     def emit_reset(self, fail_after=-1):
         """forget what filter_rewrite_tag handed to its emitter so far; fail_after >= 0: the emitter refuses from that call on"""
-        self.L.flbref_emit_reset(fail_after)
+        if self.L is not None:
+            self.L.flbref_emit_reset(fail_after)
 
+    @_recorded()
     def emitted(self):
         """[(tag, record bytes)] in the order filter_rewrite_tag called in_emitter_add_record()"""
+        return self._emitted()
+
+    @_recorded()
+    def emitted_grouped(self):
+        """the state those per-record in_emitter_add_record() calls leave in the emitter: [(tag, the records' bytes, count)],
+        one buffer per tag in the order the tags first came"""
+        d = {}
+        for t, b in self._emitted():
+            d.setdefault(t, []).append(b)
+        return [(t, b"".join(v), len(v)) for t, v in d.items()]
+
+    def _emitted(self):
         log, n = C.c_void_p(), C.c_size_t()
         self.L.flbref_emit_log(C.byref(log), C.byref(n))
         raw = C.string_at(log.value, n.value) if n.value else b""
@@ -89,6 +274,7 @@ class Ref:
             at += 8 + tl + sz
         return out
 
+    @_recorded()
     def filter_counters(self, f):
         """the instance's framework counters (src/flb_filter.c:574-616) as {metric line without timestamp}"""
         p = self.L.flbref_filter_cmt_text(f)
@@ -96,9 +282,10 @@ class Ref:
         self.L.flbref_cfree(p)
         return sorted(l.split(" ", 1)[1] for l in t.splitlines() if " " in l)
 
+    @_recorded()
     def l2m_text(self, f):
         p = self.L.flbref_l2m_cmt_text(f)
-        t = C.string_at(p).decode()
+        t = C.string_at(p).decode(errors="replace")
         self.L.flbref_cfree(p)
         return t
 
@@ -106,6 +293,7 @@ class Ref:
     def _b(s):
         return s if s is None or isinstance(s, bytes) else s.encode()
 
+    @_recorded(handle=True)
     def parser(self, name, format, regex=None, skip_empty=True, time_fmt=None, time_key=None, time_offset=None,
                time_keep=False, time_strict=True, logfmt_no_bare_keys=False, types=None, decoders=None):
         b = self._b
@@ -124,6 +312,7 @@ class Ref:
             raise RuntimeError("reference rejected parser " + name)
         return p
 
+    @_recorded()
     def parser_do(self, p, line):
         out, n = C.c_void_p(), C.c_size_t()
         s, ns = C.c_longlong(), C.c_longlong()
@@ -133,6 +322,7 @@ class Ref:
             self.L.flbref_free(out)
         return r, data, (s.value, ns.value)
 
+    @_recorded()
     def lines_to_events(self, text, key="log", skip_empty_lines=True, sec=0, nsec=0, path_key=None, path=None, offset_key=None, stream_offset=0):
         """in_tail's line loop with the reference's encoder: (chunk bytes or None, bytes consumed, lines seen)"""
         n, used, lines = C.c_size_t(), C.c_size_t(), C.c_size_t()
@@ -143,6 +333,7 @@ class Ref:
         self.L.flbref_cfree(p)
         return out, used.value, lines.value
 
+    @_recorded()
     def to_json(self, data, json_format=3, date_format=0, date_key="date", escape_unicode=True):
         """flb_pack_msgpack_to_json_format(): bytes or None.  json_format 1 json / 2 stream / 3 lines; date_format 0 double /
         1 iso8601 / 2 epoch / 3 java_sql_timestamp / 4 epoch_ms"""
@@ -155,6 +346,7 @@ class Ref:
         self.L.flbref_cfree(p)
         return out
 
+    @_recorded(handle=True)
     def ml_parser(self, name, type="regex", rules=(), match_string=None, negate=False, flush_ms=0, key_content=None,
                   key_group=None, key_pattern=None, parser=None):
         """a [MULTILINE_PARSER] section: flb_ml_parser_create() + one flb_ml_rule_create() per rule + flb_ml_parser_init()"""
@@ -170,6 +362,7 @@ class Ref:
             raise RuntimeError("reference rejected the states of multiline parser " + name)
         return m
 
+    @_recorded(handle=True)
     def filter(self, plugin, props):
         f = self.L.flbref_filter_create(self.cfg, self._b(plugin))
         for k, v in props:
@@ -178,6 +371,7 @@ class Ref:
             raise RuntimeError("reference filter init failed: %s %r" % (plugin, props))
         return f
 
+    @_recorded()
     def filter_cb(self, f, data, tag="test"):
         out, n = C.c_void_p(), C.c_size_t()
         buf = C.create_string_buffer(data, len(data))
@@ -189,6 +383,7 @@ class Ref:
                 self.L.flbref_free(out)
         return r, res
 
+    @_recorded()
     def chain_do(self, data, tag="test"):
         """flb_filter_do over every filter created on this Ref, in creation order."""
         out, n = C.c_void_p(), C.c_size_t()
