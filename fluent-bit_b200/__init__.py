@@ -54,7 +54,7 @@ EXPORTS = [
     "flbgpu_comm_unique_id", "flbgpu_comm_init", "flbgpu_l2m_allreduce",
     "flbgpu_pack_state_init", "flbgpu_pack_state_reset", "flbgpu_pack_json_state", "flbgpu_pack_json_state_batch",
     "flbgpu_ml_parser_create", "flbgpu_ml_parser_rule", "flbgpu_ml_parser_init", "flbgpu_ml_set_buffer_limit",
-    "flbgpu_msgpack_to_json_format", "flbgpu_lines_to_events", "flbgpu_chain_set_result_buffer",
+    "flbgpu_msgpack_to_json_format", "flbgpu_lines_to_events", "flbgpu_lines_to_events_parsed", "flbgpu_chain_set_result_buffer",
     "flbgpu_pool_new", "flbgpu_pool_do", "flbgpu_pool_destroy",
 ]
 
@@ -112,6 +112,8 @@ def load(path=None):
     L.flbgpu_msgpack_to_json_format.argtypes = [vp, vp, sz, C.c_int, C.c_int, cp, C.c_int, C.POINTER(vp), C.POINTER(sz), C.POINTER(sz)]
     L.flbgpu_lines_to_events.argtypes = [vp, vp, sz, cp, C.c_int, C.c_int64, C.c_int64, cp, cp, cp, C.c_uint64, C.POINTER(vp), C.POINTER(sz),
                                          C.POINTER(sz), C.POINTER(sz)]
+    L.flbgpu_lines_to_events_parsed.argtypes = [vp, vp, sz, cp, C.c_int, C.c_int64, C.c_int64, cp, cp, cp, C.c_uint64, C.POINTER(vp),
+                                                C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
     L.flbgpu_chain_set_result_buffer.argtypes = [vp, vp, sz]
     L.flbgpu_pool_new.restype = vp; L.flbgpu_pool_new.argtypes = [C.POINTER(vp), C.c_int]
     L.flbgpu_pool_do.argtypes = [vp, C.c_int, C.POINTER(vp), C.POINTER(sz), cp, C.c_int, C.POINTER(vp), C.POINTER(sz), C.POINTER(C.c_int)]
@@ -297,6 +299,22 @@ class Parser:
         if out.value:
             _libc.free(out)
         return r, data, (t.tv_sec, t.tv_nsec)
+
+    def lines_to_events(self, text, key="log", skip_empty_lines=True, sec=0, nsec=0, path_key=None, path=None, offset_key=None,
+                        stream_offset=0):
+        """in_tail's line loop with this parser as its `Parser`: (chunk bytes or None, bytes consumed, lines seen)"""
+        out, n, used, lines = C.c_void_p(), C.c_size_t(), C.c_size_t(), C.c_size_t()
+        buf = C.create_string_buffer(text, len(text))
+        r = self.ctx.L.flbgpu_lines_to_events_parsed(self.h, C.cast(buf, C.c_void_p), len(text), _b(key), int(skip_empty_lines), sec, nsec,
+                                                     _b(path_key), _b(path), _b(offset_key), stream_offset, C.byref(out), C.byref(n),
+                                                     C.byref(used), C.byref(lines))
+        if r < 0:
+            raise FlbGpuError("lines_to_events_parsed: %s" % self.ctx.err())
+        chunk = None
+        if out.value:
+            chunk = C.string_at(out.value, n.value)
+            _libc.free(out)
+        return chunk, used.value, lines.value
 
 
 def _parser_do_batch(self, lines):

@@ -216,6 +216,14 @@ int bk_ln_count(bk_q *q, const struct ln_env *e);
 int bk_ln_fill(bk_q *q, const struct ln_env *e, const uint64_t *d_bsum);
 int bk_ln_sizes(bk_q *q, const struct ln_env *e);
 int bk_ln_emit(bk_q *q, const struct ln_env *e, const uint64_t *d_bsum, uint8_t *d_out);
+/* ... with a parser, asynchronous on the queue's stream.  mid_size: t->msize[k] per line, kept lines counted in t->ln.n_events;
+ * mid_emit: line k's event of the parser's input at t->mid + t->mbsum[k / BK_REC_BLOCK] + (sizes before it in its block);
+ * sizes (after the parser's chain has run): t->r_out[] per record, then t->rec[k] and t->size[k] per line (*t->bad counts the
+ * lines without a record); emit: line k's event at d_out + d_bsum[k / BK_REC_BLOCK] + (sizes before it in its block). */
+int bk_tl_mid_size(bk_q *q, const struct tl_env *t);
+int bk_tl_mid_emit(bk_q *q, const struct tl_env *t);
+int bk_tl_sizes(bk_q *q, const struct tl_env *t);
+int bk_tl_emit(bk_q *q, const struct tl_env *t, const uint64_t *d_bsum, uint8_t *d_out);
 
 #ifdef __cplusplus
 }

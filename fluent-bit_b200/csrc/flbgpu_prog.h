@@ -394,6 +394,26 @@ struct ln_env {
     const uint8_t *strs;              /* key, path_key, path, offset_key, back to back */
     uint32_t key_off, key_len, path_key_off, path_key_len, path_off, path_len, offset_key_off, offset_key_len;   /* _len 0xffffffff: absent */
 };
+/* ... with a parser (in_tail's `Parser`): every kept line goes through the parser's chain as the event {"_": line}; the events are
+ * then made from the chain's result and the parser's report */
+#define TL_NONE 0xffffffffu
+struct tl_env {
+    struct ln_env ln;                 /* the text, its line feeds, the call's strings and time (ln.size: unused) */
+    uint32_t *msize;                  /* bytes of line k's event in the parser's input (0: stepped over) */
+    const uint64_t *mbsum;            /* ... their offsets per BK_REC_BLOCK lines */
+    uint8_t *mid;                     /* the parser's input: one event per kept line, back to back */
+    const uint32_t *r_off, *r_len;    /* the chain's record index over `mid` (kind 2: an event-shaped piece inside a line) */
+    const uint8_t *r_kind;
+    uint32_t n_rec;
+    const uint32_t *r_size;           /* bytes of record r in the chain's result, */
+    const uint64_t *r_bsum;           /* ... their offsets per BK_REC_BLOCK records */
+    uint32_t *r_out;                  /* record r's offset in the result */
+    const uint8_t *res;               /* the chain's result */
+    const int32_t *prep;              /* the parser's report: 6 ints per record (parsed, position, seconds lo / hi, nanoseconds, -) */
+    uint32_t *rec;                    /* the record of line k (TL_NONE: stepped over) */
+    uint32_t *size;                   /* bytes of line k's event */
+    uint32_t *bad;                    /* lines whose event is not where the chain's index has a record */
+};
 
 /* ---------------------------------------------------- streaming JSON packer (dev_jsmn.cuh) */
 enum { JM_UNDEFINED = 0, JM_OBJECT = 1, JM_ARRAY = 2, JM_STRING = 4, JM_PRIMITIVE = 8 };     /* jsmntype_t, lib/jsmn/jsmn.h */

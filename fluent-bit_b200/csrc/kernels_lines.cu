@@ -5,6 +5,11 @@
  *                  by a shuffle scan inside the block)
  *   k_ln_size .... one lane per line: what the line keeps, the size of its event; lines that became events counted per block
  *   k_ln_emit .... one lane per line: the event at its offset
+ * With a parser (flbgpu_lines_to_events_parsed):
+ *   k_tl_mid_size / k_tl_mid_emit ... one lane per line: its event {"_": line} in the parser's input
+ *   k_tl_roff .... one lane per record of the parser's chain: where its result starts
+ *   k_tl_size .... one lane per line: its record (found by offset in the chain's index), the bytes of its event
+ *   k_tl_emit .... one lane per line: the event at its offset, from the chain's result and the parser's report
  * Byte-stream work bounded by HBM traffic (text in once per pass, events out once): no tensor cores.  The functions are in
  * dev_lines.cuh, shared with the CPU emulation of the tests.  A translation unit of its own.
  */
@@ -64,6 +69,53 @@ __global__ void __launch_bounds__(BK_REC_BLOCK) k_ln_emit(const __grid_constant_
     if (sz) ln_emit(&e, k, out + bsum[blockIdx.x] + ex);
 }
 
+/* with a parser (tl_*): the parser's input, the result offsets of the chain's records, the events */
+__global__ void __launch_bounds__(BK_REC_BLOCK) k_tl_mid_size(const __grid_constant__ tl_env t)
+{
+    const uint32_t k = blockIdx.x * BK_REC_BLOCK + threadIdx.x;
+    uint32_t sz = 0;
+    if (k < t.ln.n_lines) { sz = tl_mid_size(&t, k); t.msize[k] = sz; }
+    const int made = __syncthreads_count(sz != 0);
+    if (threadIdx.x == 0 && made) atomicAdd(t.ln.n_events, (unsigned long long) made);
+}
+__global__ void __launch_bounds__(BK_REC_BLOCK) k_tl_mid_emit(const __grid_constant__ tl_env t)
+{
+    const uint32_t k = blockIdx.x * BK_REC_BLOCK + threadIdx.x;
+    const uint32_t sz = k < t.ln.n_lines ? t.msize[k] : 0u;
+    const uint32_t ex = ln_block_excl(sz);
+    if (sz) tl_mid_emit(&t, k, t.mid + t.mbsum[blockIdx.x] + ex);
+}
+__global__ void __launch_bounds__(BK_REC_BLOCK) k_tl_roff(const __grid_constant__ tl_env t)
+{
+    const uint32_t r = blockIdx.x * BK_REC_BLOCK + threadIdx.x;
+    const uint32_t sz = r < t.n_rec ? t.r_size[r] : 0u;
+    const uint32_t ex = ln_block_excl(sz);
+    if (r < t.n_rec) t.r_out[r] = (uint32_t) (t.r_bsum[blockIdx.x] + ex);
+}
+__global__ void __launch_bounds__(BK_REC_BLOCK) k_tl_size(const __grid_constant__ tl_env t)
+{
+    const uint32_t k = blockIdx.x * BK_REC_BLOCK + threadIdx.x;
+    const uint32_t ms = k < t.ln.n_lines ? t.msize[k] : 0u;
+    const uint32_t ex = ln_block_excl(ms);
+    if (k < t.ln.n_lines) {
+        uint32_t r = TL_NONE, sz = 0;
+        if (ms) {
+            r = tl_find(&t, (uint32_t) (t.mbsum[blockIdx.x] + ex), ms);
+            if (r != TL_NONE) sz = tl_event(&t, k, r, 0);
+            if (!sz) atomicAdd(t.bad, 1u);
+        }
+        t.rec[k] = sz ? r : TL_NONE;
+        t.size[k] = sz;
+    }
+}
+__global__ void __launch_bounds__(BK_REC_BLOCK) k_tl_emit(const __grid_constant__ tl_env t, const uint64_t *__restrict__ bsum, uint8_t *__restrict__ out)
+{
+    const uint32_t k = blockIdx.x * BK_REC_BLOCK + threadIdx.x;
+    const uint32_t sz = k < t.ln.n_lines ? t.size[k] : 0u;
+    const uint32_t ex = ln_block_excl(sz);
+    if (sz) tl_event(&t, k, t.rec[k], out + bsum[blockIdx.x] + ex);
+}
+
 #define LN_GRID(n) (((n) + BK_REC_BLOCK - 1) / BK_REC_BLOCK)
 #define LN_ST(q) ((cudaStream_t) bk_stream(q))
 
@@ -104,6 +156,47 @@ int bk_ln_emit(bk_q *q, const struct ln_env *e, const uint64_t *d_bsum, uint8_t 
     CKL(cudaSetDevice(bk_q_device(q)));
     bk_ev_begin(q, 2);
     k_ln_emit<<<LN_GRID(e->n_lines), BK_REC_BLOCK, 0, LN_ST(q)>>>(*e, d_bsum, d_out);
+    bk_ev_end(q, 2);
+    bk_note_launches(1);
+    CKL(cudaGetLastError());
+    return 0;
+}
+
+int bk_tl_mid_size(bk_q *q, const struct tl_env *t)
+{
+    if (!t->ln.n_lines) return 0;
+    CKL(cudaSetDevice(bk_q_device(q)));
+    k_tl_mid_size<<<LN_GRID(t->ln.n_lines), BK_REC_BLOCK, 0, LN_ST(q)>>>(*t);
+    bk_note_launches(1);
+    CKL(cudaGetLastError());
+    return 0;
+}
+int bk_tl_mid_emit(bk_q *q, const struct tl_env *t)
+{
+    if (!t->ln.n_lines) return 0;
+    CKL(cudaSetDevice(bk_q_device(q)));
+    k_tl_mid_emit<<<LN_GRID(t->ln.n_lines), BK_REC_BLOCK, 0, LN_ST(q)>>>(*t);
+    bk_note_launches(1);
+    CKL(cudaGetLastError());
+    return 0;
+}
+int bk_tl_sizes(bk_q *q, const struct tl_env *t)
+{
+    CKL(cudaSetDevice(bk_q_device(q)));
+    bk_ev_begin(q, 2);
+    if (t->n_rec) k_tl_roff<<<LN_GRID(t->n_rec), BK_REC_BLOCK, 0, LN_ST(q)>>>(*t);
+    if (t->ln.n_lines) k_tl_size<<<LN_GRID(t->ln.n_lines), BK_REC_BLOCK, 0, LN_ST(q)>>>(*t);
+    bk_ev_end(q, 2);
+    bk_note_launches(2);
+    CKL(cudaGetLastError());
+    return 0;
+}
+int bk_tl_emit(bk_q *q, const struct tl_env *t, const uint64_t *d_bsum, uint8_t *d_out)
+{
+    if (!t->ln.n_lines) return 0;
+    CKL(cudaSetDevice(bk_q_device(q)));
+    bk_ev_begin(q, 2);
+    k_tl_emit<<<LN_GRID(t->ln.n_lines), BK_REC_BLOCK, 0, LN_ST(q)>>>(*t, d_bsum, d_out);
     bk_ev_end(q, 2);
     bk_note_launches(1);
     CKL(cudaGetLastError());

@@ -211,6 +211,11 @@ struct flbgpu_chain {
     uint32_t active;                          /* bit k: filter k is routed this call's tag (Match / Match_Regex / active) */
     uint32_t spec_active;                     /* the routing the speculation belongs to */
     uint32_t small_cap_rec; size_t small_cap_out;   /* what the small-chunk form learnt about this instance's chunks */
+    int keep_result;                          /* the device-output form without a caller's buffer: the result stays in d_out */
+    /* flbgpu_lines_to_events_parsed() on a parser's chain: the text, the lines and the parser's input live apart from every
+     * buffer chain_run() grows, since growing one frees memory queued kernels may still read */
+    uint8_t *d_tl_text, *d_tl_mid, *d_tl_out; uint32_t *d_tl_line, *d_tl_rec; uint64_t *d_tl_bsum, *h_tl_bsum;
+    size_t cap_tl_text, cap_tl_mid, cap_tl_out, cap_tl_line, cap_tl_rec, cap_tl_bsum, cap_tl_hbsum;
     struct flbgpu_stats st;
 };
 
@@ -1555,6 +1560,8 @@ void flbgpu_chain_destroy(flbgpu_chain *c)
     bk_free(c->q, c->d_len); bk_free(c->q, c->d_size); bk_free(c->q, c->d_kind); bk_free(c->q, c->d_bsum); bk_free(c->q, c->d_cap);
     bk_free(c->q, c->d_flags); bk_free(c->q, c->d_scr); free(c->h_bsum); bk_free(c->q, c->d_mlw);
     bk_free(c->q, c->d_prep); free(c->h_prep);
+    bk_free(c->q, c->d_tl_text); bk_free(c->q, c->d_tl_mid); bk_free(c->q, c->d_tl_out); bk_free(c->q, c->d_tl_line); bk_free(c->q, c->d_tl_rec);
+    bk_free(c->q, c->d_tl_bsum); free(c->h_tl_bsum);
     bk_free(c->q, c->d_esize); bk_free(c->q, c->d_ebsum); free(c->h_ebsum);
     bk_free(c->q, c->l2m.hash); bk_free(c->q, c->l2m.chash); bk_free(c->q, c->l2m.first); bk_free(c->q, c->l2m.cnt); bk_free(c->q, c->l2m.sum); bk_free(c->q, c->l2m.bkt); bk_free(c->q, c->l2m.str); bk_free(c->q, c->l2m.pending); bk_free(c->q, c->l2m.pending_n);
     free(c->h_hash); free(c->h_chash); free(c->h_first); free(c->h_cnt); free(c->h_sum); free(c->h_bkt);
@@ -2111,6 +2118,7 @@ static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_e
 
     /* ---- emit (+ download) ---- */
     if (!host_out) {
+        if (!ext_out && c->keep_result) { GROW(c->d_out, c->cap_out, total, uint8_t); ext_out = c->d_out; ext_cap = c->cap_out; }
         if (ext_cap < total) { set_err("device output buffer too small%s%s", NULL, NULL); return -1; }
         if (bk_chain_emit(c->q, &a, ext_out, 0, nb)) return -1;
     }

@@ -143,6 +143,22 @@ int flbgpu_msgpack_to_json_format(flbgpu_ctx *ctx, const void *data, size_t byte
 int flbgpu_lines_to_events(flbgpu_ctx *ctx, const char *text, size_t bytes, const char *key, int skip_empty_lines,
                            int64_t sec, int64_t nsec, const char *path_key, const char *path, const char *offset_key,
                            uint64_t stream_offset, void **out_buf, size_t *out_size, size_t *consumed, size_t *lines);
+/* The same loop with in_tail's `Parser` set (tail_file.c:721-746): arguments and results as flbgpu_lines_to_events(), the
+ * context is the parser's.  For every line the loop keeps:
+ *   1. the parser gets the line without its trailing '\r' (as the plain event carries it);
+ *   2. when it parses (flb_parser_do() >= 0), the event is flb_tail_pack_line_map()'s (:281-336):
+ *      `[[time, {}], {<the parsed map's members, each re-encoded as msgpack_pack_object() writes it>, [path_key: path,]
+ *      [offset_key: stream_offset + offset of the line]}]` -- path and offset come AFTER the parsed members, and a parsed key
+ *      equal to path_key appears twice.  The time is the parsed one; when flb_time_to_nanosec() of it is 0 (no time key, or
+ *      exactly the epoch) it is the call's sec / nsec.  Seconds and nanoseconds go out as (uint32_t), like the encoder's;
+ *   3. when it does not parse, the event is the plain one with the call's time, but of the line as read: a trailing '\r' stays;
+ *   4. the parser is flb_parser_do() whole: every format, Types, Time_Keep, Time_Offset, the decoders, Skip_Empty_Values;
+ *   5. a line the device refuses to parse (FLBGPU_E_RXSTACK, RXBUDGET, RXUNICODE, FIELDS, FLOAT, DEEP, ...) fails the call:
+ *      -1, flbgpu_last_error() names the bits.  Such a line never becomes a rule-3 event, since the reference would parse it.
+ * Calls with the same parser take turns (its flbgpu_parser_do() chain does the work); different parsers run side by side. */
+int flbgpu_lines_to_events_parsed(flbgpu_parser *parser, const char *text, size_t bytes, const char *key, int skip_empty_lines,
+                                  int64_t sec, int64_t nsec, const char *path_key, const char *path, const char *offset_key,
+                                  uint64_t stream_offset, void **out_buf, size_t *out_size, size_t *consumed, size_t *lines);
 
 /* ---- multiline parser definitions ----------------------------------------------------------------------------
  * What a [MULTILINE_PARSER] section becomes (src/flb_parser.c:815-935): flb_ml_parser_create()
