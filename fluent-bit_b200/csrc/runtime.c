@@ -1589,8 +1589,49 @@ int flbgpu_kernel_ms(flbgpu_ctx *ctx, float out[3])
     return bk_kernel_ms(q, out);
 }
 
-#define GROW(ptr, cap, need, type) do { if ((cap) < (size_t) (need)) { size_t nc_ = (size_t) (need) + (size_t) (need) / 4 + 64; \
-        bk_free(c->q, ptr); (ptr) = (type *) bk_alloc(c->q, nc_ * sizeof(type)); if (!(ptr)) { (cap) = 0; return -1; } (cap) = nc_; } } while (0)
+/* grow a device buffer of `elem`-byte elements to hold n of them (n + n/4 + 64, and bk_alloc's tail), keeping its first
+ * `keep` elements.  The queue drains first: kernels queued on it may still read the old buffer. */
+static int dev_grow(flbgpu_chain *c, void **p, size_t *cap, size_t n, size_t elem, size_t keep)
+{
+    size_t nc = n + n / 4 + 64;
+    void *np;
+    if (*cap >= n) return 0;
+    if (bk_sync(c->q)) return -1;
+    np = bk_alloc(c->q, nc * elem);
+    if (!np || (keep && bk_d2d(c->q, np, *p, keep * elem))) { bk_free(c->q, np); return -1; }
+    bk_free(c->q, *p);
+    *p = np; *cap = nc;
+    return 0;
+}
+
+/* the same for a host array, whose contents never need to move */
+static int host_grow(void **p, size_t *cap, size_t n, size_t elem)
+{
+    size_t nc = n + n / 4 + 64;
+    if (*cap >= n) return 0;
+    free(*p);
+    *p = malloc(nc * elem);
+    *cap = *p ? nc : 0;
+    if (!*p) { set_err("out of memory%s%s", NULL, NULL); return -1; }
+    return 0;
+}
+
+/* per-record sizes -> block offsets, on the device (d_bsum) and the host (h_bsum); *total = the sum of the n sizes.  NULL
+ * arrays: the chain's own, grown to fit.  A total of 4 GiB or more fails the call with the text `too_big`. */
+static int sizes_to_offsets(flbgpu_chain *c, const uint32_t *d_size, uint32_t n, uint64_t *d_bsum, uint64_t *h_bsum,
+                            const char *too_big, uint64_t *total)
+{
+    const size_t nb = ((size_t) n + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
+    if (!d_bsum) {
+        if (dev_grow(c, (void **) &c->d_bsum, &c->cap_bsum, nb + 2, sizeof(uint64_t), 0) ||
+            host_grow((void **) &c->h_bsum, &c->cap_hbsum, nb + 2, sizeof(uint64_t))) return -1;
+        d_bsum = c->d_bsum; h_bsum = c->h_bsum;
+    }
+    if (bk_sizes_scan(c->q, d_size, n, d_bsum, h_bsum)) return -1;
+    *total = h_bsum[nb];
+    if (*total >= 0xfff00000ull) { set_err("%s%s", too_big, NULL); return -1; }
+    return 0;
+}
 
 /* chunk-level verdict of filter k from the evidence word (see dev_chain.cuh).
  * `clean`: the filter's input decodes to its very end.  grep and modify return
@@ -1610,6 +1651,22 @@ static int verdict(int kind, uint32_t fl, int clean)
 }
 /* log_to_metrics: MODIFIED (empty) iff discard_logs, whatever the records were */
 #define L2M_VERDICT(c, k) ((c)->f[k]->l2m->discard ? 1 : 0)
+
+/* the chunk-level verdicts of a call from its evidence words, front to back.  Returns the first filter whose verdict differs
+ * from `assume` (the filters behind it saw the wrong input), or -1.  *settled = `assume` with that verdict in place, which is
+ * also what the next call speculates on. */
+static int settle(flbgpu_chain *c, uint32_t assume, const uint32_t *flags, int clean, uint32_t *settled)
+{
+    int k;
+    for (k = 0; k < c->nf; k++) {
+        const int v = !((c->active >> k) & 1) ? 0 : c->f[k]->kind == FLBGPU_F_LOG_TO_METRICS ? L2M_VERDICT(c, k) : verdict(c->f[k]->kind, flags[k], clean);
+        if (v) clean = 1;                    /* a MODIFIED filter hands a well-formed chunk on */
+        if (v != (int) ((assume >> k) & 1)) { assume ^= 1u << k; break; }
+    }
+    *settled = assume;
+    c->spec_assume = assume; c->spec_valid = 1; c->spec_active = c->active;
+    return k < c->nf ? k : -1;
+}
 
 /* grow the per-record arrays to hold `need` records, keeping the first `keep` */
 static int ensure_rec_cap(flbgpu_chain *c, size_t need, size_t keep)
@@ -1658,6 +1715,47 @@ static size_t slice_bytes(void)
     if (mb < 1) mb = 1;
     if (mb > 2048) mb = 2048;
     return mb << 20;
+}
+
+/* the record index of the slice [off, off + len) of a chunk, behind the n_rec records indexed so far: *n_valid more records,
+ * and the slice's decodable part ends at *end_off */
+static int index_slice(flbgpu_chain *c, const uint8_t *d_in, size_t off, size_t len, uint32_t n_rec, uint32_t *n_valid, uint64_t *end_off)
+{
+    /* tiles start at the address rounded down to 16 B */
+    const uint32_t n_tiles = (uint32_t) ((len + ((uintptr_t) (d_in + off) & 15) + BK_INDEX_TILE - 1) / BK_INDEX_TILE);
+    uint32_t n_cand = 0;
+    int tiled = 0;
+    *n_valid = 0; *end_off = off;
+    if (bk_upload_wait_index(c->q, off + len)) return -1;
+    if (dev_grow(c, (void **) &c->d_tile, &c->cap_tile, n_tiles + 1, sizeof(uint32_t), 0)) return -1;
+    if (bk_index_count(c->q, d_in, off, (uint32_t) len, c->d_tile, n_tiles, &n_cand)) return -1;
+    if (ensure_rec_cap(c, (size_t) n_rec + n_cand, n_rec)) return -1;
+    if (bk_index_fill(c->q, d_in, off, (uint32_t) len, c->d_tile, n_tiles, n_cand, c->d_off + n_rec, c->d_len + n_rec,
+                      c->d_kind + n_rec, n_valid, end_off, &tiled)) {
+        c->st.error_bits = FLBGPU_E_INDEX;
+        return -1;
+    }
+    return 0;
+}
+
+/* the record index of a whole chunk, slice by slice: *n_rec records, whose decodable prefix ends at *off */
+static int index_chunk(flbgpu_chain *c, const uint8_t *d_in, size_t bytes, uint32_t *n_rec, size_t *off)
+{
+    size_t S = slice_bytes();
+    *n_rec = 0; *off = 0;
+    while (*off < bytes) {
+        size_t len = bytes - *off < S ? bytes - *off : S;
+        uint32_t n_valid;
+        uint64_t end_off;
+        if (index_slice(c, d_in, *off, len, *n_rec, &n_valid, &end_off)) return -1;
+        if (n_valid == 0) {
+            if (*off + len < bytes) { S *= 2; continue; }     /* a record longer than the slice: widen it */
+            break;                                           /* nothing decodable from here to the end */
+        }
+        *n_rec += n_valid;
+        *off = (size_t) end_off;
+    }
+    return 0;
 }
 
 static void fill_args(flbgpu_chain *c, struct bk_chain_args *a, const uint8_t *d_in, size_t bytes, uint32_t n_rec)
@@ -2001,6 +2099,39 @@ static int rtag_collect(flbgpu_chain *c, const struct bk_chain_args *a, uint32_t
     return 0;
 }
 
+/* the host buffer a result of `need` bytes goes to: the caller's (flbgpu_chain_set_result_buffer) while it fits, else a
+ * malloc() of `size` bytes; res_drop() releases it on failure */
+static void *res_take(flbgpu_chain *c, size_t need, size_t size)
+{
+    return (c->res_buf && c->res_cap >= need) ? (void *) c->res_buf : malloc(size);
+}
+static void res_drop(flbgpu_chain *c, void *p)
+{
+    if ((uint8_t *) p != c->res_buf) free(p);
+}
+
+static void hugepage_hint(void *p, size_t n)
+{
+#ifdef MADV_HUGEPAGE
+    const char *e = getenv("FLBGPU_HUGEPAGE");
+    if (e && e[0] == '0') return;
+    if (n >= ((size_t) 8 << 20)) {                    /* fewer, larger page faults while the result is filled in */
+        uintptr_t lo = ((uintptr_t) p + ((size_t) 2 << 20) - 1) & ~(((uintptr_t) 2 << 20) - 1);
+        uintptr_t hi = ((uintptr_t) p + n) & ~(((uintptr_t) 2 << 20) - 1);
+        if (hi > lo) madvise((void *) lo, hi - lo, MADV_HUGEPAGE);
+    }
+#else
+    (void) p; (void) n;
+#endif
+}
+
+static float ms_since(const struct timespec *t0)
+{
+    struct timespec t1;
+    clock_gettime(CLOCK_MONOTONIC, &t1);
+    return (float) ((t1.tv_sec - t0->tv_sec) * 1e3 + (t1.tv_nsec - t0->tv_nsec) / 1e6);
+}
+
 static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_ext, size_t bytes,
                      uint8_t *ext_out, size_t ext_cap, void **host_out, size_t *out_size)
 {
@@ -2009,23 +2140,21 @@ static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_e
     uint32_t n_rec = 0, h_flags[FLBGPU_MAX_FILTERS + 1], nb;
     size_t off = 0, S = slice_bytes();
     uint64_t total;
-    int clean, k, pass;
+    int clean, pass;
+    struct timespec t0;
 
-    struct timespec t0, t1;
     memset(&c->st, 0, sizeof(c->st));
     c->st.bytes_in = bytes;
     *out_size = 0;
     clock_gettime(CLOCK_MONOTONIC, &t0);
-#define PHASE_MARK(i) do { clock_gettime(CLOCK_MONOTONIC, &t1); \
-        c->st.phase_ms[i] = (float) ((t1.tv_sec - t0.tv_sec) * 1e3 + (t1.tv_nsec - t0.tv_nsec) / 1e6); } while (0)
     if (bytes >= 0xfff00000ull) { set_err("chunk larger than 4 GiB: split the append%s%s", NULL, NULL); return -1; }
     if (d_in_ext) { d_in = d_in_ext; bk_upload_none(c->q); }
     else {
-        GROW(c->d_in, c->cap_in, bytes + 64, uint8_t);
+        if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0)) return -1;
         d_in = c->d_in;
         if (bk_upload_start(c->q, c->d_in, h_in, bytes)) return -1;
     }
-    if (c->needs_scratch) GROW(c->d_scr, c->cap_scr, (size_t) c->scr_mul * bytes + 64, uint8_t);
+    if (c->needs_scratch && dev_grow(c, (void **) &c->d_scr, &c->cap_scr, (size_t) c->scr_mul * bytes + 64, 1, 0)) return -1;
     memset(&a, 0, sizeof(a));
     a.now = (int64_t) time(NULL);
     a.assume = initial_assume(c);
@@ -2034,26 +2163,14 @@ static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_e
     /* ---- index + evaluate, slice by slice, while the upload is still running ---- */
     while (off < bytes) {
         size_t len = bytes - off < S ? bytes - off : S;
-        uint32_t n_tiles = (uint32_t) ((len + ((uintptr_t) (d_in + off) & 15) + BK_INDEX_TILE - 1) / BK_INDEX_TILE), n_cand = 0, n_valid = 0;   /* tiles start at the address rounded down to 16 B */
-        uint64_t end_off = off;
-        uint32_t assume = a.assume;
-        int64_t now = a.now;
-        int tiled = 0;
-        if (bk_upload_wait_index(c->q, off + len)) return -1;
-        GROW(c->d_tile, c->cap_tile, n_tiles + 1, uint32_t);
-        if (bk_index_count(c->q, d_in, off, (uint32_t) len, c->d_tile, n_tiles, &n_cand)) return -1;
-        if (ensure_rec_cap(c, (size_t) n_rec + n_cand, n_rec)) return -1;
-        if (bk_index_fill(c->q, d_in, off, (uint32_t) len, c->d_tile, n_tiles, n_cand, c->d_off + n_rec, c->d_len + n_rec,
-                          c->d_kind + n_rec, &n_valid, &end_off, &tiled)) {
-            c->st.error_bits = FLBGPU_E_INDEX;
-            return -1;
-        }
+        uint32_t n_valid;
+        uint64_t end_off;
+        if (index_slice(c, d_in, off, len, n_rec, &n_valid, &end_off)) return -1;
         if (n_valid == 0) {
             if (off + len < bytes) { S *= 2; continue; }       /* a record longer than the slice: widen it */
             break;                                             /* nothing decodable from here to the end */
         }
         fill_args(c, &a, d_in, bytes, n_rec + n_valid);
-        a.assume = assume; a.now = now;
         bk_hint_streaming(c->q, a.d_in + off, (size_t) end_off - off);
         if (bk_chain_eval(c->q, &a, n_rec, n_rec + n_valid)) return -1;
         n_rec += n_valid;
@@ -2063,94 +2180,64 @@ static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_e
     REFUSE_WIDE_ARRAYS(h_in, d_in, return -1);
     c->st.records_in = n_rec;
     c->st.passes = 1;
-    {
-        uint32_t assume = a.assume;
-        int64_t now = a.now;
-        fill_args(c, &a, d_in, bytes, n_rec);
-        a.assume = assume; a.now = now;
-    }
+    fill_args(c, &a, d_in, bytes, n_rec);
 
     /* ---- chunk-level verdicts; revise assumptions front to back until they hold ---- */
     for (pass = 0; pass <= c->nf; pass++) {
-        int changed = 0, cl = clean;
         if (bk_flags_fetch(c->q, c->d_flags, h_flags)) return -1;
         if (refused(c, h_flags[FLBGPU_MAX_FILTERS])) return -1;
-        for (k = 0; k < c->nf; k++) {
-            int v = !((c->active >> k) & 1) ? 0 : c->f[k]->kind == FLBGPU_F_LOG_TO_METRICS ? L2M_VERDICT(c, k) : verdict(c->f[k]->kind, h_flags[k], cl);
-            if (v) cl = 1;                   /* a MODIFIED filter hands a well-formed chunk on */
-            if (v != (int) ((a.assume >> k) & 1)) {
-                a.assume = (a.assume & ~(1u << k)) | ((uint32_t) v << k);
-                changed = 1;
-                break;                       /* later filters saw the wrong input: re-evaluate */
-            }
-        }
-        if (!changed) break;
+        if (settle(c, a.assume, h_flags, clean, &a.assume) < 0) break;
+        /* later filters saw the wrong input: re-evaluate */
         if (bk_flags_clear(c->q, c->d_flags) || l2m_clear(c) || report_clear(c) || bk_chain_eval(c->q, &a, 0, n_rec)) return -1;
         c->st.passes++;
     }
     c->st.kernel_launches = bk_launch_count();
-    PHASE_MARK(0);
-    c->spec_assume = a.assume; c->spec_valid = 1; c->spec_active = c->active;    /* what the streaming path speculates on next time */
+    c->st.phase_ms[0] = ms_since(&t0);
     if (l2m_merge(c)) return -1;
-    nb = (n_rec + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
-    GROW(c->d_bsum, c->cap_bsum, nb + 2, uint64_t);
-    if (c->cap_hbsum < (size_t) nb + 2) {
-        free(c->h_bsum);
-        c->cap_hbsum = (size_t) nb + nb / 4 + 64;
-        c->h_bsum = malloc(c->cap_hbsum * sizeof(uint64_t));
-        if (!c->h_bsum) { c->cap_hbsum = 0; return -1; }
-    }
-    a.d_bsum = c->d_bsum;
     /* the records a rewrite_tag filter matched go to its emitter whatever the filter's own verdict is (a chunk that does not
      * decode to its end makes it NOTOUCH after the fact, rewrite_tag.c:500-546) */
     if (a.d_esize && rtag_collect(c, &a, n_rec, (h_flags[c->rtag_index] & CHF_CAUSE) != 0)) return -1;
     if (a.assume == 0) return FLBGPU_FILTER_NOTOUCH;
 
     /* ---- output offsets ---- */
-    if (bk_sizes_scan(c->q, c->d_size, n_rec, c->d_bsum, c->h_bsum)) return -1;
-    total = c->h_bsum[nb];
-    if (total >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); return -1; }
+    if (sizes_to_offsets(c, c->d_size, n_rec, NULL, NULL, "result larger than 4 GiB", &total)) return -1;
+    a.d_bsum = c->d_bsum;
+    nb = (n_rec + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
     c->st.bytes_out = total;
     *out_size = (size_t) total;
-    PHASE_MARK(1);
-    c->st.phase_ms[1] -= c->st.phase_ms[0];
+    c->st.phase_ms[1] = ms_since(&t0) - c->st.phase_ms[0];
     if (total == 0) return FLBGPU_FILTER_MODIFIED;
 
     /* ---- emit (+ download) ---- */
     if (!host_out) {
-        if (!ext_out && c->keep_result) { GROW(c->d_out, c->cap_out, total, uint8_t); ext_out = c->d_out; ext_cap = c->cap_out; }
+        if (!ext_out && c->keep_result) {
+            if (dev_grow(c, (void **) &c->d_out, &c->cap_out, total, 1, 0)) return -1;
+            ext_out = c->d_out; ext_cap = c->cap_out;
+        }
         if (ext_cap < total) { set_err("device output buffer too small%s%s", NULL, NULL); return -1; }
         if (bk_chain_emit(c->q, &a, ext_out, 0, nb)) return -1;
     }
     else {
         const uint32_t step = 2048;                   /* blocks per emission launch (512 K records) */
         uint32_t b0;
-        void *out = (c->res_buf && c->res_cap >= total) ? (void *) c->res_buf : malloc((size_t) total);
+        void *out = res_take(c, total, total);
         if (!out) return -1;
-#define RES_FREE(p_) do { if ((uint8_t *) (p_) != c->res_buf) free(p_); } while (0)
-#ifdef MADV_HUGEPAGE
-        if ((uint8_t *) out != c->res_buf && total >= ((size_t) 8 << 20)) {            /* fewer, larger page faults while the result is filled in */
-            uintptr_t lo = ((uintptr_t) out + ((size_t) 2 << 20) - 1) & ~(((uintptr_t) 2 << 20) - 1);
-            uintptr_t hi = ((uintptr_t) out + (size_t) total) & ~(((uintptr_t) 2 << 20) - 1);
-            if (hi > lo) madvise((void *) lo, hi - lo, MADV_HUGEPAGE);
-        }
-#endif
-        GROW(c->d_out, c->cap_out, total, uint8_t);
-        if (bk_download_begin(c->q, out, c->d_out)) { RES_FREE(out); return -1; }
+        if ((uint8_t *) out != c->res_buf) hugepage_hint(out, total);
+        if (dev_grow(c, (void **) &c->d_out, &c->cap_out, total, 1, 0) || bk_download_begin(c->q, out, c->d_out)) { res_drop(c, out); return -1; }
         for (b0 = 0; b0 < nb; b0 += step) {
             uint32_t b1 = b0 + step < nb ? b0 + step : nb;
             if (bk_chain_emit(c->q, &a, c->d_out, b0, b1) || bk_download_push(c->q, (size_t) c->h_bsum[b0], (size_t) c->h_bsum[b1])) {
                 bk_download_end(c->q);
-                RES_FREE(out);
+                res_drop(c, out);
                 return -1;
             }
         }
-        if (bk_download_end(c->q)) { RES_FREE(out); return -1; }
+        if (bk_download_end(c->q)) { res_drop(c, out); return -1; }
         *host_out = out;
     }
     c->st.kernel_launches = bk_launch_count();
     if (host_out) bk_records_out(c->q, &c->st.records_out);     /* (the device-output form leaves the stream running) */
-    PHASE_MARK(3);
+    c->st.phase_ms[3] = ms_since(&t0);
     c->st.phase_ms[2] = c->st.phase_ms[3] - c->st.phase_ms[1] - c->st.phase_ms[0];
     return FLBGPU_FILTER_MODIFIED;
 }
@@ -2189,21 +2276,6 @@ void flbgpu_stream_copy(void *dst, const void *src, size_t n)
     memcpy(dst, src, n);
 }
 
-static void hugepage_hint(void *p, size_t n)
-{
-#ifdef MADV_HUGEPAGE
-    const char *e = getenv("FLBGPU_HUGEPAGE");
-    if (e && e[0] == '0') return;
-    if (n >= ((size_t) 8 << 20)) {                    /* fewer, larger page faults while the result is filled in */
-        uintptr_t lo = ((uintptr_t) p + ((size_t) 2 << 20) - 1) & ~(((uintptr_t) 2 << 20) - 1);
-        uintptr_t hi = ((uintptr_t) p + n) & ~(((uintptr_t) 2 << 20) - 1);
-        if (hi > lo) madvise((void *) lo, hi - lo, MADV_HUGEPAGE);
-    }
-#else
-    (void) p; (void) n;
-#endif
-}
-
 /* Streaming form of chain_run for host buffers.  The chunk-level verdicts are only known when the
  * whole chunk has been evaluated, but they almost never differ from the previous call's (and from
  * "every filter modifies" on the first call), so each slice is emitted and sent back as soon as it
@@ -2218,9 +2290,8 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
     const int taper = !(getenv("FLBGPU_TAPER") && getenv("FLBGPU_TAPER")[0] == '0');
     uint64_t placed = 0;
     uint8_t *out = NULL;
-    int clean, k, dl_open = 0, rc = -1;
-    int64_t now = (int64_t) time(NULL);
-    struct timespec t0, t1;
+    int clean, dl_open = 0;
+    struct timespec t0;
 
     memset(&c->st, 0, sizeof(c->st));
     c->st.bytes_in = bytes;
@@ -2230,24 +2301,21 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
     if (c->spec_valid && c->spec_active == c->active) assume = c->spec_assume;
     if (assume == 0) return 1;                       /* nothing would be emitted: the classic path decides */
     if (bytes >= 0xfff00000ull) { set_err("chunk larger than 4 GiB: split the append%s%s", NULL, NULL); return -1; }
-    GROW(c->d_in, c->cap_in, bytes + 64, uint8_t);
+    if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0)) return -1;
     if (bk_upload_start(c->q, c->d_in, h_in, bytes)) return -1;
-    if (c->needs_scratch) GROW(c->d_scr, c->cap_scr, (size_t) c->scr_mul * bytes + 64, uint8_t);
+    if (c->needs_scratch && dev_grow(c, (void **) &c->d_scr, &c->cap_scr, (size_t) c->scr_mul * bytes + 64, 1, 0)) return -1;
     nb_max = (uint32_t) (bytes / (3 * BK_REC_BLOCK)) + 4;       /* an event is at least 3 bytes */
-    GROW(c->d_bsum, c->cap_bsum, nb_max, uint64_t);
-    if (c->cap_hbsum < (size_t) nb_max) {
-        free(c->h_bsum);
-        c->cap_hbsum = nb_max;
-        c->h_bsum = malloc(c->cap_hbsum * sizeof(uint64_t));
-        if (!c->h_bsum) { c->cap_hbsum = 0; return -1; }
-    }
+    if (dev_grow(c, (void **) &c->d_bsum, &c->cap_bsum, nb_max, sizeof(uint64_t), 0) ||
+        host_grow((void **) &c->h_bsum, &c->cap_hbsum, nb_max, sizeof(uint64_t))) return -1;
     memset(&a, 0, sizeof(a));
+    a.now = (int64_t) time(NULL);
+    a.assume = assume;
     if (bk_flags_clear(c->q, c->d_flags) || l2m_clear(c) || report_clear(c)) return -1;
 
 #define STREAM_FLUSH(upto_blocks) do { \
         uint32_t b1_ = (upto_blocks); \
         if (b1_ > b_done) { \
-            fill_args(c, &a, c->d_in, bytes, n_rec); a.assume = assume; a.now = now; a.d_bsum = c->d_bsum; \
+            fill_args(c, &a, c->d_in, bytes, n_rec); \
             if (bk_sizes_scan_range(c->q, c->d_size, n_rec, b_done, b1_, c->d_bsum, c->h_bsum, placed)) goto fail; \
             if (c->h_bsum[b1_] >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); goto fail; } \
             if (c->h_bsum[b1_] > placed) { \
@@ -2258,13 +2326,15 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
                     uint8_t *no_; \
                     if (want_ < c->h_bsum[b1_]) want_ = (size_t) c->h_bsum[b1_] + ((size_t) 8 << 20); \
                     if (dl_open) { if (bk_download_end(c->q)) { dl_open = 0; goto fail; } dl_open = 0; } \
-                    if (!out && c->res_buf && c->res_cap >= c->h_bsum[b1_]) { no_ = c->res_buf; want_ = c->res_cap; }   /* the caller's buffer, while the result fits */ \
-                    else if (out == c->res_buf && out) { no_ = malloc(want_); if (no_) memcpy(no_, out, (size_t) placed); }           /* outgrown: what has arrived moves */ \
+                    if (!out) no_ = res_take(c, (size_t) c->h_bsum[b1_], want_); \
+                    else if (out == c->res_buf) { no_ = malloc(want_); if (no_) memcpy(no_, out, (size_t) placed); }           /* outgrown: what has arrived moves */ \
                     else no_ = realloc(out, want_); \
                     if (!no_) goto fail; \
+                    if (no_ == c->res_buf) want_ = c->res_cap; \
                     out = no_; cap_out_h = want_; \
                     if (out != c->res_buf) hugepage_hint(out, want_); \
-                    GROW_KEEP_OUT(want_); \
+                    /* the device output buffer grows with the host one; bytes already emitted stay where they are */ \
+                    if (dev_grow(c, (void **) &c->d_out, &c->cap_out, want_, 1, (size_t) placed)) goto fail; \
                 } \
                 if (!dl_open) { if (bk_download_begin(c->q, out, c->d_out)) goto fail; dl_open = 1; } \
                 if (bk_chain_emit(c->q, &a, c->d_out, b_done, b1_) || bk_download_push(c->q, (size_t) placed, (size_t) c->h_bsum[b1_])) goto fail; \
@@ -2272,32 +2342,17 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
             placed = c->h_bsum[b1_]; \
             b_done = b1_; \
         } } while (0)
-    /* the device output buffer grows with the host one; bytes already emitted stay where they are */
-#define GROW_KEEP_OUT(need) do { if (c->cap_out < (size_t) (need)) { \
-        uint8_t *nd_ = bk_alloc(c->q, (size_t) (need) + 64); \
-        if (!nd_) goto fail; \
-        if (placed) { if (bk_sync(c->q) || bk_d2d(c->q, nd_, c->d_out, (size_t) placed)) { bk_free(c->q, nd_); goto fail; } } \
-        bk_free(c->q, c->d_out); c->d_out = nd_; c->cap_out = (size_t) (need); } } while (0)
 
     while (off < bytes) {
         /* slices shrink towards the end of the chunk: what is left to do after the last upload piece
          * arrives (index, evaluate, emit, download of the last slice) is proportional to its size */
         size_t rem = bytes - off, want = S, len;
+        uint32_t n_valid;
+        uint64_t end_off;
         if (taper && rem < 3 * S) { want = rem / 3; if (want < ((size_t) 16 << 20)) want = (size_t) 16 << 20; if (want > S) want = S; }
         if (want < force) want = force;
         len = rem < want ? rem : want;
-        uint32_t n_tiles = (uint32_t) ((len + ((uintptr_t) (c->d_in + off) & 15) + BK_INDEX_TILE - 1) / BK_INDEX_TILE), n_cand = 0, n_valid = 0;
-        uint64_t end_off = off;
-        int tiled = 0;
-        if (bk_upload_wait_index(c->q, off + len)) goto fail;
-        GROW(c->d_tile, c->cap_tile, n_tiles + 1, uint32_t);
-        if (bk_index_count(c->q, c->d_in, off, (uint32_t) len, c->d_tile, n_tiles, &n_cand)) goto fail;
-        if (ensure_rec_cap(c, (size_t) n_rec + n_cand, n_rec)) goto fail;
-        if (bk_index_fill(c->q, c->d_in, off, (uint32_t) len, c->d_tile, n_tiles, n_cand, c->d_off + n_rec, c->d_len + n_rec,
-                          c->d_kind + n_rec, &n_valid, &end_off, &tiled)) {
-            c->st.error_bits = FLBGPU_E_INDEX;
-            goto fail;
-        }
+        if (index_slice(c, c->d_in, off, len, n_rec, &n_valid, &end_off)) goto fail;
         if (n_valid == 0) {
             if (off + len < bytes) { force = 2 * len; continue; }   /* a record longer than the slice: widen it */
             break;
@@ -2306,7 +2361,6 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
         /* the previous slice has been evaluated by now (or is about to finish): place and send it */
         STREAM_FLUSH(n_rec / BK_REC_BLOCK);
         fill_args(c, &a, c->d_in, bytes, n_rec + n_valid);
-        a.assume = assume; a.now = now;
         bk_hint_streaming(c->q, a.d_in + off, (size_t) end_off - off);
         if (bk_chain_eval(c->q, &a, n_rec, n_rec + n_valid)) goto fail;
         n_rec += n_valid;
@@ -2322,52 +2376,37 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
     /* ---- the verdicts must be the ones speculated on ---- */
     if (bk_flags_fetch(c->q, c->d_flags, h_flags)) goto fail;
     if (refused(c, h_flags[FLBGPU_MAX_FILTERS])) goto fail;
-    {
-        int cl = clean;
-        uint32_t settled = 0;
-        for (k = 0; k < c->nf; k++) {
-            int v = !((c->active >> k) & 1) ? 0 : c->f[k]->kind == FLBGPU_F_LOG_TO_METRICS ? L2M_VERDICT(c, k) : verdict(c->f[k]->kind, h_flags[k], cl);
-            if (v) cl = 1;
-            if (v != (int) ((assume >> k) & 1)) {
-                /* evidence of the later filters was gathered under a wrong assumption: redo classically,
-                 * and speculate on "filter k as found" next time */
-                c->spec_assume = (assume & ~(1u << k)) | ((uint32_t) v << k);
-                c->spec_valid = 1; c->spec_active = c->active;
-                if (dl_open) bk_download_end(c->q);
-                free(out);
-                return 1;
-            }
-            settled |= (uint32_t) v << k;
-        }
-        c->spec_assume = settled; c->spec_valid = 1; c->spec_active = c->active;
+    if (settle(c, assume, h_flags, clean, &assume) >= 0) {
+        /* evidence of the later filters was gathered under a wrong assumption: redo classically (the next call
+         * speculates on the verdict as found) */
+        if (dl_open) bk_download_end(c->q);
+        res_drop(c, out);
+        return 1;
     }
     c->st.kernel_launches = bk_launch_count();
     if (l2m_merge(c)) goto fail;
     if (dl_open) { dl_open = 0; if (bk_download_end(c->q)) goto fail; }
     if (c->rtag_index >= 0 && ((c->active >> c->rtag_index) & 1)) {      /* every record of the call is still indexed: one re-tagged stream */
-        fill_args(c, &a, c->d_in, bytes, n_rec); a.assume = assume; a.now = now;
+        fill_args(c, &a, c->d_in, bytes, n_rec);
         if (rtag_collect(c, &a, n_rec, (h_flags[c->rtag_index] & CHF_CAUSE) != 0)) goto fail;
     }
     bk_records_out(c->q, &c->st.records_out);
     c->st.bytes_out = placed;
     *out_size = (size_t) placed;
-    if (placed == 0) { RES_FREE(out); out = NULL; }
+    if (placed == 0) { res_drop(c, out); out = NULL; }
     else if (out != c->res_buf && cap_out_h > placed + placed / 2) {     /* badly over-estimated: give the excess back */
         uint8_t *sh = realloc(out, (size_t) placed);
         if (sh) out = sh;
     }
     *host_out = out;
-    clock_gettime(CLOCK_MONOTONIC, &t1);
-    c->st.phase_ms[3] = (float) ((t1.tv_sec - t0.tv_sec) * 1e3 + (t1.tv_nsec - t0.tv_nsec) / 1e6);
+    c->st.phase_ms[3] = ms_since(&t0);
     *ret = FLBGPU_FILTER_MODIFIED;
     return 0;
 fail:
     if (dl_open) bk_download_end(c->q);
-    RES_FREE(out);
-    (void) rc;
+    res_drop(c, out);
     return -1;
 #undef STREAM_FLUSH
-#undef GROW_KEEP_OUT
 }
 
 /* One append as flb_filter_do() hands it over (tens of KB to a few MB): the whole call is one stream of work
@@ -2392,8 +2431,8 @@ static int chain_run_small(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, v
     struct bk_small_res res;
     uint32_t assume, n_tiles, cap_rec, nb_cap;
     size_t off, cap_out;
-    int clean, k;
-    struct timespec t0, t1;
+    int clean;
+    struct timespec t0;
 
     assume = initial_assume(c);
     if (c->spec_valid && c->spec_active == c->active) assume = c->spec_assume;
@@ -2408,17 +2447,17 @@ static int chain_run_small(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, v
     if (c->small_cap_rec > cap_rec) cap_rec = c->small_cap_rec;
     nb_cap = (cap_rec + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
     n_tiles = (uint32_t) ((bytes + BK_INDEX_TILE - 1) / BK_INDEX_TILE);
-    GROW(c->d_in, c->cap_in, bytes + 64, uint8_t);
-    if (c->needs_scratch) GROW(c->d_scr, c->cap_scr, (size_t) c->scr_mul * bytes + 64, uint8_t);
-    GROW(c->d_tile, c->cap_tile, n_tiles + 1, uint32_t);
-    GROW(c->d_bsum, c->cap_bsum, nb_cap + 2, uint64_t);
-    if (ensure_rec_cap(c, cap_rec, 0)) return -1;
     cap_out = bytes + bytes / 2 + 4096;
     if (c->small_cap_out > cap_out) cap_out = c->small_cap_out;
-    GROW(c->d_out, c->cap_out, cap_out, uint8_t);
+    if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0) ||
+        (c->needs_scratch && dev_grow(c, (void **) &c->d_scr, &c->cap_scr, (size_t) c->scr_mul * bytes + 64, 1, 0)) ||
+        dev_grow(c, (void **) &c->d_tile, &c->cap_tile, n_tiles + 1, sizeof(uint32_t), 0) ||
+        dev_grow(c, (void **) &c->d_bsum, &c->cap_bsum, nb_cap + 2, sizeof(uint64_t), 0) ||
+        ensure_rec_cap(c, cap_rec, 0) ||
+        dev_grow(c, (void **) &c->d_out, &c->cap_out, cap_out, 1, 0)) return -1;
     cap_out = c->cap_out;
     fill_args(c, &a, c->d_in, bytes, 0);
-    a.assume = assume; a.now = (int64_t) time(NULL); a.d_bsum = c->d_bsum;
+    a.assume = assume; a.now = (int64_t) time(NULL);
     if (bk_flags_clear(c->q, c->d_flags) || l2m_clear(c) || report_clear(c)) return -1;
     if (bk_small_run(c->q, &a, h_in, c->d_in, bytes, cap_rec, c->d_tile, n_tiles, c->d_out, cap_out, &res)) return -1;
     c->st.kernel_launches = bk_launch_count();
@@ -2432,25 +2471,11 @@ static int chain_run_small(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, v
     c->st.records_in = res.n_valid;
     c->st.passes = 1;
     if (refused(c, res.flags[FLBGPU_MAX_FILTERS])) return -1;
-    {
-        int cl = clean;
-        uint32_t settled = 0;
-        for (k = 0; k < c->nf; k++) {
-            int v = !((c->active >> k) & 1) ? 0 : c->f[k]->kind == FLBGPU_F_LOG_TO_METRICS ? L2M_VERDICT(c, k) : verdict(c->f[k]->kind, res.flags[k], cl);
-            if (v) cl = 1;
-            if (v != (int) ((assume >> k) & 1)) {
-                c->spec_assume = (assume & ~(1u << k)) | ((uint32_t) v << k);
-                c->spec_valid = 1; c->spec_active = c->active;
-                return 1;
-            }
-            settled |= (uint32_t) v << k;
-        }
-        c->spec_assume = settled; c->spec_valid = 1; c->spec_active = c->active;
-    }
+    if (settle(c, assume, res.flags, clean, &assume) >= 0) return 1;
     if (l2m_merge(c)) return -1;
     if (res.total >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); return -1; }
     if (res.emitted && c->rtag_index >= 0 && ((c->active >> c->rtag_index) & 1)) {
-        fill_args(c, &a, c->d_in, bytes, res.n_valid); a.assume = assume;
+        fill_args(c, &a, c->d_in, bytes, res.n_valid);
         if (rtag_collect(c, &a, res.n_valid, (res.flags[c->rtag_index] & CHF_CAUSE) != 0)) return -1;
     }
     if (!res.emitted) {                              /* the result outgrew the output buffer: remember, let the general path do this call */
@@ -2462,13 +2487,12 @@ static int chain_run_small(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, v
     *out_size = (size_t) res.total;
     *host_out = NULL;
     if (res.total) {
-        void *out = (c->res_buf && c->res_cap >= res.total) ? (void *) c->res_buf : malloc((size_t) res.total);
+        void *out = res_take(c, (size_t) res.total, (size_t) res.total);
         if (!out) { set_err("out of memory%s%s", NULL, NULL); return -1; }
-        if (bk_small_fetch(c->q, out, c->d_out, (size_t) res.total)) { RES_FREE(out); return -1; }
+        if (bk_small_fetch(c->q, out, c->d_out, (size_t) res.total)) { res_drop(c, out); return -1; }
         *host_out = out;
     }
-    clock_gettime(CLOCK_MONOTONIC, &t1);
-    c->st.phase_ms[3] = (float) ((t1.tv_sec - t0.tv_sec) * 1e3 + (t1.tv_nsec - t0.tv_nsec) / 1e6);
+    c->st.phase_ms[3] = ms_since(&t0);
     *ret = FLBGPU_FILTER_MODIFIED;
     return 0;
 }
@@ -2780,12 +2804,7 @@ static size_t put_line_event(uint8_t *rec, const char *buf, size_t length)
 static const int32_t *parser_report(flbgpu_chain *c, uint32_t n)
 {
     if (c->st.records_in != n) { set_err("parser call: the lines did not come back one to one%s%s", NULL, NULL); return NULL; }
-    if (c->cap_hprep < (size_t) n * 6) {
-        free(c->h_prep);
-        c->cap_hprep = (size_t) n * 6 + 64;
-        c->h_prep = malloc(c->cap_hprep * sizeof(int32_t));
-        if (!c->h_prep) { c->cap_hprep = 0; set_err("out of memory%s%s", NULL, NULL); return NULL; }
-    }
+    if (host_grow((void **) &c->h_prep, &c->cap_hprep, (size_t) n * 6, sizeof(int32_t))) return NULL;
     if (bk_d2h(c->q, c->h_prep, c->d_prep, (size_t) n * 6 * sizeof(int32_t)) || bk_sync(c->q)) return NULL;
     return c->h_prep;
 }

@@ -1,6 +1,51 @@
 /* runtime_lines.h -- host side of the raw text -> log events conversion (part of runtime.c, included there).
  * The line loop of in_tail: plugins/in_tail/tail_file.c:629-700, :338-391. */
 
+/* the arguments both line calls take: checked, the outputs cleared, the call's constants and strings in *e, the strings packed
+ * into strs (*n_strs bytes, 1 KB at most).  1: nothing to do (no text); -1: refused */
+static int ln_args(struct ln_env *e, uint8_t *strs, size_t *n_strs, const char *text, size_t bytes, const char *key, int skip_empty_lines,
+                   int64_t sec, int64_t nsec, const char *path_key, const char *path, const char *offset_key, uint64_t stream_offset,
+                   void **out_buf, size_t *out_size, size_t *consumed, size_t *lines)
+{
+    size_t at = 0;
+    if (!out_buf || !out_size || !key || (!text && bytes)) return -1;
+    *out_buf = NULL; *out_size = 0;
+    if (consumed) *consumed = 0;
+    if (lines) *lines = 0;
+    if (bytes == 0) return 1;
+    if (bytes >= 0xfff00000ull) { set_err("more than 4 GiB of text in one call%s%s", NULL, NULL); return -1; }
+    if ((path_key && !path) || strlen(key) + (path_key ? strlen(path_key) + strlen(path) : 0) + (offset_key ? strlen(offset_key) : 0) > 1024) {
+        set_err("key / path_key / path / offset_key: missing or longer than 1 KB together%s%s", NULL, NULL);
+        return -1;
+    }
+    e->bytes = bytes; e->sec = sec; e->nsec = nsec; e->skip_empty_lines = skip_empty_lines ? 1u : 0u; e->stream_offset = stream_offset;
+#define LN_STR(s, off_field, len_field) do { if (s) { e->off_field = (uint32_t) at; e->len_field = (uint32_t) strlen(s); memcpy(strs + at, s, e->len_field); at += e->len_field; } \
+        else e->len_field = 0xffffffffu; } while (0)
+    LN_STR(key, key_off, key_len);
+    LN_STR(path_key, path_key_off, path_key_len);
+    if (path_key) LN_STR(path, path_off, path_len); else e->path_len = 0xffffffffu;
+    LN_STR(offset_key, offset_key_off, offset_key_len);
+#undef LN_STR
+    e->n_tiles = (uint32_t) ((bytes + LN_TILE - 1) / LN_TILE);
+    *n_strs = at;
+    return 0;
+}
+
+/* the text and the strings to e->text / e->strs, then the line feeds counted per tile and placed: e->n_lines, the tile offsets
+ * in d_tiles / h_bsum (NULL: the chain's own).  All on the compute stream, where the line kernels run: the staged upload
+ * (bk_upload_start) orders only the index stream, so the counting pass could read text that has not arrived and the filling
+ * pass write more line feeds than were counted. */
+static int ln_count_lines(flbgpu_chain *c, struct ln_env *e, const char *text, const uint8_t *strs, size_t n_strs,
+                          uint64_t *d_tiles, uint64_t *h_bsum)
+{
+    uint64_t n;
+    if (bk_h2d(c->q, (void *) e->text, text, e->bytes) || bk_h2d(c->q, (void *) e->strs, strs, n_strs ? n_strs : 1) ||
+        bk_zero(c->q, e->n_events, 16) || bk_ln_count(c->q, e) ||
+        sizes_to_offsets(c, e->cnt, e->n_tiles, d_tiles, h_bsum, "too many lines in one call", &n)) return -1;
+    e->n_lines = (uint32_t) n;
+    return 0;
+}
+
 int flbgpu_lines_to_events(flbgpu_ctx *ctx, const char *text, size_t bytes, const char *key, int skip_empty_lines,
                            int64_t sec, int64_t nsec, const char *path_key, const char *path, const char *offset_key,
                            uint64_t stream_offset, void **out_buf, size_t *out_size, size_t *consumed, size_t *lines)
@@ -8,95 +53,50 @@ int flbgpu_lines_to_events(flbgpu_ctx *ctx, const char *text, size_t bytes, cons
     flbgpu_chain *c;
     struct ln_env e;
     uint8_t strs[1024];
-    uint32_t nbt, nbl, last_nl = 0;
+    uint32_t last_nl = 0;
     unsigned long long n_events = 0;
-    size_t at = 0, need;
+    size_t n_strs = 0;
     uint64_t total;
-    int r = -1;
+    int r;
     g_rt_err[0] = 0;
-    if (!ctx || !out_buf || !out_size || !key || (!text && bytes)) return -1;
-    *out_buf = NULL; *out_size = 0;
-    if (consumed) *consumed = 0;
-    if (lines) *lines = 0;
-    if (bytes == 0) return 0;
-    if (bytes >= 0xfff00000ull) { set_err("more than 4 GiB of text in one call%s%s", NULL, NULL); return -1; }
-    if ((path_key && !path) || strlen(key) + (path_key ? strlen(path_key) + strlen(path) : 0) + (offset_key ? strlen(offset_key) : 0) > sizeof(strs)) {
-        set_err("key / path_key / path / offset_key: missing or longer than 1 KB together%s%s", NULL, NULL);
-        return -1;
-    }
+    if (!ctx) return -1;
+    memset(&e, 0, sizeof(e));
+    r = ln_args(&e, strs, &n_strs, text, bytes, key, skip_empty_lines, sec, nsec, path_key, path, offset_key, stream_offset,
+                out_buf, out_size, consumed, lines);
+    if (r) return r < 0 ? -1 : 0;
     c = tj_chain(ctx);
     if (!c) return -1;
     pthread_mutex_lock(&c->lock);
     ctx->last_q = c->q;
-    memset(&e, 0, sizeof(e));
-    e.bytes = bytes; e.sec = sec; e.nsec = nsec; e.skip_empty_lines = skip_empty_lines ? 1u : 0u; e.stream_offset = stream_offset;
-#define LN_STR(s, off_field, len_field) do { if (s) { e.off_field = (uint32_t) at; e.len_field = (uint32_t) strlen(s); memcpy(strs + at, s, e.len_field); at += e.len_field; } \
-        else e.len_field = 0xffffffffu; } while (0)
-    LN_STR(key, key_off, key_len);
-    LN_STR(path_key, path_key_off, path_key_len);
-    if (path_key) LN_STR(path, path_off, path_len); else e.path_len = 0xffffffffu;
-    LN_STR(offset_key, offset_key_off, offset_key_len);
-#undef LN_STR
-    e.n_tiles = (uint32_t) ((bytes + LN_TILE - 1) / LN_TILE);
-    nbt = (e.n_tiles + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
 #define LN_FAIL() do { bk_upload_end(c->q); pthread_mutex_unlock(&c->lock); return -1; } while (0)
-#define LN_GROW(ptr, cap, n_, type) do { if ((cap) < (size_t) (n_)) { size_t nc_ = (size_t) (n_) + (size_t) (n_) / 4 + 64; \
-        bk_free(c->q, ptr); (ptr) = (type *) bk_alloc(c->q, nc_ * sizeof(type)); if (!(ptr)) { (cap) = 0; LN_FAIL(); } (cap) = nc_; } } while (0)
-    LN_GROW(c->d_in, c->cap_in, bytes + 64, uint8_t);
-    /* on the compute stream, where the line kernels run: the staged upload (bk_upload_start) orders only the index stream, so
-     * the counting pass could read text that has not arrived and the filling pass write more line feeds than were counted */
-    if (bk_h2d(c->q, c->d_in, text, bytes)) LN_FAIL();
+    /* the text; work memory: the strings, the counts per tile; the line arrays once the number of lines is known */
+    if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0) ||
+        dev_grow(c, (void **) &c->d_mlw, &c->cap_mlw, 1024 + 16 + sizeof(uint32_t) * (size_t) e.n_tiles + 64, 1, 0)) LN_FAIL();
     e.text = c->d_in;
-    /* work memory: the strings, the counts per tile; the line arrays once the number of lines is known */
-    need = 1024 + 16 + sizeof(uint32_t) * (size_t) e.n_tiles + 64;
-    LN_GROW(c->d_mlw, c->cap_mlw, need, uint8_t);
     e.strs = c->d_mlw;
     e.n_events = (unsigned long long *) (c->d_mlw + 1024);
     e.cnt = (uint32_t *) (c->d_mlw + 1024 + 16);
-    if (bk_zero(c->q, e.n_events, 16)) LN_FAIL();
-    LN_GROW(c->d_bsum, c->cap_bsum, nbt + 2, uint64_t);
-    if (c->cap_hbsum < (size_t) nbt + 2) {
-        free(c->h_bsum);
-        c->cap_hbsum = (size_t) nbt + nbt / 4 + 64;
-        c->h_bsum = malloc(c->cap_hbsum * sizeof(uint64_t));
-        if (!c->h_bsum) { c->cap_hbsum = 0; LN_FAIL(); }
-    }
-    if (bk_h2d(c->q, c->d_mlw, strs, at ? at : 1) || bk_ln_count(c->q, &e) || bk_sizes_scan(c->q, e.cnt, e.n_tiles, c->d_bsum, c->h_bsum)) LN_FAIL();
-    if (c->h_bsum[nbt] >= 0xfff00000ull) { set_err("too many lines in one call%s%s", NULL, NULL); LN_FAIL(); }
-    e.n_lines = (uint32_t) c->h_bsum[nbt];
+    if (ln_count_lines(c, &e, text, strs, n_strs, NULL, NULL)) LN_FAIL();
     bk_upload_end(c->q);
     c->st.records_in = e.n_lines;
     if (e.n_lines == 0) { pthread_mutex_unlock(&c->lock); return 0; }               /* no complete line yet */
     if (ensure_rec_cap(c, e.n_lines, 0)) LN_FAIL();
     e.nl = c->d_off; e.size = c->d_size;                                            /* (the record arrays of the chain, by another name) */
-    if (bk_ln_fill(c->q, &e, c->d_bsum)) LN_FAIL();
-    nbl = (e.n_lines + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
-    LN_GROW(c->d_bsum, c->cap_bsum, nbl + 2, uint64_t);                             /* (ln_fill has run: the tile offsets are not needed again... */
-    if (c->cap_hbsum < (size_t) nbl + 2) {
-        free(c->h_bsum);
-        c->cap_hbsum = (size_t) nbl + nbl / 4 + 64;
-        c->h_bsum = malloc(c->cap_hbsum * sizeof(uint64_t));
-        if (!c->h_bsum) { c->cap_hbsum = 0; LN_FAIL(); }
-    }
-    if (bk_sync(c->q)) LN_FAIL();                                                    /* ... once it has really run) */
-    if (bk_ln_sizes(c->q, &e) || bk_sizes_scan(c->q, e.size, e.n_lines, c->d_bsum, c->h_bsum)) LN_FAIL();
-    total = c->h_bsum[nbl];
-    if (total >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); LN_FAIL(); }
+    if (bk_ln_fill(c->q, &e, c->d_bsum) || bk_ln_sizes(c->q, &e) ||
+        sizes_to_offsets(c, e.size, e.n_lines, NULL, NULL, "result larger than 4 GiB", &total)) LN_FAIL();
     if (bk_d2h(c->q, &last_nl, e.nl + (e.n_lines - 1), sizeof(last_nl)) || bk_d2h(c->q, &n_events, e.n_events, sizeof(n_events)) || bk_sync(c->q)) LN_FAIL();
     if (consumed) *consumed = (size_t) last_nl + 1;
     if (lines) *lines = (size_t) n_events;                                          /* (`lines` of the reference counts what reached go_next) */
-    r = 0;
     if (total) {
         void *out = malloc((size_t) total);
         if (!out) LN_FAIL();
-        LN_GROW(c->d_out, c->cap_out, total, uint8_t);
-        if (bk_ln_emit(c->q, &e, c->d_bsum, c->d_out) || bk_d2h(c->q, out, c->d_out, (size_t) total) || bk_sync(c->q)) { free(out); LN_FAIL(); }
+        if (dev_grow(c, (void **) &c->d_out, &c->cap_out, total, 1, 0) || bk_ln_emit(c->q, &e, c->d_bsum, c->d_out) ||
+            bk_d2h(c->q, out, c->d_out, (size_t) total) || bk_sync(c->q)) { free(out); LN_FAIL(); }
         *out_buf = out; *out_size = (size_t) total;
     }
     c->st.bytes_in = bytes; c->st.bytes_out = total; c->st.kernel_launches = bk_launch_count();
     pthread_mutex_unlock(&c->lock);
-    return r;
-#undef LN_GROW
+    return 0;
 #undef LN_FAIL
 }
 
@@ -134,78 +134,51 @@ int flbgpu_lines_to_events_parsed(flbgpu_parser *p, const char *text, size_t byt
     struct tl_env t;
     struct ln_env *e = &t.ln;
     uint8_t strs[1024];
-    uint32_t nbt, nbl, nbl_max, last_nl = 0, bad = 0, h_flags[FLBGPU_MAX_FILTERS + 1];
+    uint32_t nbt, nbl_max, last_nl = 0, bad = 0, h_flags[FLBGPU_MAX_FILTERS + 1];
     unsigned long long n_events = 0;
-    size_t at = 0, text_room, osz = 0;
+    size_t n_strs = 0, text_room, osz = 0;
     uint64_t *d_tiles, *d_fbsum, mid_total, total;
     int r;
     g_rt_err[0] = 0;
-    if (!p || !out_buf || !out_size || !key || (!text && bytes)) return -1;
-    *out_buf = NULL; *out_size = 0;
-    if (consumed) *consumed = 0;
-    if (lines) *lines = 0;
-    if (bytes == 0) return 0;
-    if (bytes >= 0xfff00000ull) { set_err("more than 4 GiB of text in one call%s%s", NULL, NULL); return -1; }
-    if ((path_key && !path) || strlen(key) + (path_key ? strlen(path_key) + strlen(path) : 0) + (offset_key ? strlen(offset_key) : 0) > sizeof(strs)) {
-        set_err("key / path_key / path / offset_key: missing or longer than 1 KB together%s%s", NULL, NULL);
-        return -1;
-    }
+    if (!p) return -1;
+    memset(&t, 0, sizeof(t));
+    r = ln_args(e, strs, &n_strs, text, bytes, key, skip_empty_lines, sec, nsec, path_key, path, offset_key, stream_offset,
+                out_buf, out_size, consumed, lines);
+    if (r) return r < 0 ? -1 : 0;
     if (parser_solo(p)) return -1;
     c = p->solo;
     pthread_mutex_lock(&c->lock);
     p->ctx->last_q = c->q;
     c->active = 1;
-    memset(&t, 0, sizeof(t));
-    e->bytes = bytes; e->sec = sec; e->nsec = nsec; e->skip_empty_lines = skip_empty_lines ? 1u : 0u; e->stream_offset = stream_offset;
-#define LN_STR(s, off_field, len_field) do { if (s) { e->off_field = (uint32_t) at; e->len_field = (uint32_t) strlen(s); memcpy(strs + at, s, e->len_field); at += e->len_field; } \
-        else e->len_field = 0xffffffffu; } while (0)
-    LN_STR(key, key_off, key_len);
-    LN_STR(path_key, path_key_off, path_key_len);
-    if (path_key) LN_STR(path, path_off, path_len); else e->path_len = 0xffffffffu;
-    LN_STR(offset_key, offset_key_off, offset_key_len);
-#undef LN_STR
-    e->n_tiles = (uint32_t) ((bytes + LN_TILE - 1) / LN_TILE);
     nbt = (e->n_tiles + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
     nbl_max = (uint32_t) ((bytes + BK_REC_BLOCK - 1) / BK_REC_BLOCK);          /* (a line takes one byte at least: its '\n') */
 #define TL_FAIL() do { c->keep_result = 0; pthread_mutex_unlock(&c->lock); return -1; } while (0)
-#define TL_GROW(ptr, cap, n_, type) do { if ((cap) < (size_t) (n_)) { size_t nc_ = (size_t) (n_) + (size_t) (n_) / 4 + 64; \
-        if (bk_sync(c->q)) { TL_FAIL(); } bk_free(c->q, ptr); (ptr) = (type *) bk_alloc(c->q, nc_ * sizeof(type)); if (!(ptr)) { (cap) = 0; TL_FAIL(); } (cap) = nc_; } } while (0)
     /* the text, then the strings, the counters (events, lines without a record) and the line feeds per tile */
     text_room = (bytes + 64 + 15) & ~(size_t) 15;
-    TL_GROW(c->d_tl_text, c->cap_tl_text, text_room + 1024 + 16 + sizeof(uint32_t) * (size_t) e->n_tiles, uint8_t);
+    if (dev_grow(c, (void **) &c->d_tl_text, &c->cap_tl_text, text_room + 1024 + 16 + sizeof(uint32_t) * (size_t) e->n_tiles, 1, 0)) TL_FAIL();
     e->text = c->d_tl_text;
     e->strs = c->d_tl_text + text_room;
     e->n_events = (unsigned long long *) (c->d_tl_text + text_room + 1024);
     t.bad = (uint32_t *) (c->d_tl_text + text_room + 1024 + 8);
     e->cnt = (uint32_t *) (c->d_tl_text + text_room + 1024 + 16);
     /* block offsets: of the tiles, of the parser's input per line, of the events per line */
-    TL_GROW(c->d_tl_bsum, c->cap_tl_bsum, (size_t) nbt + 2 + 2 * ((size_t) nbl_max + 2), uint64_t);
+    if (dev_grow(c, (void **) &c->d_tl_bsum, &c->cap_tl_bsum, (size_t) nbt + 2 + 2 * ((size_t) nbl_max + 2), sizeof(uint64_t), 0) ||
+        host_grow((void **) &c->h_tl_bsum, &c->cap_tl_hbsum, (size_t) (nbt > nbl_max ? nbt : nbl_max) + 2, sizeof(uint64_t))) TL_FAIL();
     d_tiles = c->d_tl_bsum;
     t.mbsum = c->d_tl_bsum + nbt + 2;
     d_fbsum = c->d_tl_bsum + nbt + 2 + nbl_max + 2;
-    if (c->cap_tl_hbsum < (size_t) (nbt > nbl_max ? nbt : nbl_max) + 2) {
-        free(c->h_tl_bsum);
-        c->cap_tl_hbsum = (size_t) (nbt > nbl_max ? nbt : nbl_max) + 2;
-        c->h_tl_bsum = malloc(c->cap_tl_hbsum * sizeof(uint64_t));
-        if (!c->h_tl_bsum) { c->cap_tl_hbsum = 0; set_err("out of memory%s%s", NULL, NULL); TL_FAIL(); }
-    }
-    if (bk_h2d(c->q, c->d_tl_text, text, bytes) || bk_h2d(c->q, (void *) e->strs, strs, at ? at : 1) || bk_zero(c->q, e->n_events, 16) ||
-        bk_ln_count(c->q, e) || bk_sizes_scan(c->q, e->cnt, e->n_tiles, d_tiles, c->h_tl_bsum)) TL_FAIL();
-    if (c->h_tl_bsum[nbt] >= 0xfff00000ull) { set_err("too many lines in one call%s%s", NULL, NULL); TL_FAIL(); }
-    e->n_lines = (uint32_t) c->h_tl_bsum[nbt];
+    if (ln_count_lines(c, e, text, strs, n_strs, d_tiles, c->h_tl_bsum)) TL_FAIL();
     if (e->n_lines == 0) { pthread_mutex_unlock(&c->lock); return 0; }             /* no complete line yet */
-    nbl = (e->n_lines + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
     /* per line: line feed, bytes in the parser's input, record, bytes of the event */
-    TL_GROW(c->d_tl_line, c->cap_tl_line, 4 * (size_t) e->n_lines, uint32_t);
+    if (dev_grow(c, (void **) &c->d_tl_line, &c->cap_tl_line, 4 * (size_t) e->n_lines, sizeof(uint32_t), 0)) TL_FAIL();
     e->nl = c->d_tl_line;
     t.msize = c->d_tl_line + e->n_lines;
     t.rec = c->d_tl_line + 2 * (size_t) e->n_lines;
     t.size = c->d_tl_line + 3 * (size_t) e->n_lines;
-    if (bk_ln_fill(c->q, e, d_tiles) || bk_tl_mid_size(c->q, &t) || bk_sizes_scan(c->q, t.msize, e->n_lines, (uint64_t *) t.mbsum, c->h_tl_bsum)) TL_FAIL();
-    mid_total = c->h_tl_bsum[nbl];
-    if (mid_total >= 0xfff00000ull) { set_err("parser input larger than 4 GiB%s%s", NULL, NULL); TL_FAIL(); }
+    if (bk_ln_fill(c->q, e, d_tiles) || bk_tl_mid_size(c->q, &t) ||
+        sizes_to_offsets(c, t.msize, e->n_lines, (uint64_t *) t.mbsum, c->h_tl_bsum, "parser input larger than 4 GiB", &mid_total)) TL_FAIL();
     if (mid_total) {
-        TL_GROW(c->d_tl_mid, c->cap_tl_mid, mid_total + 64, uint8_t);
+        if (dev_grow(c, (void **) &c->d_tl_mid, &c->cap_tl_mid, mid_total + 64, 1, 0)) TL_FAIL();
         t.mid = c->d_tl_mid;
         /* the chain's index kernels run on a stream of their own: the parser's input is complete before they start */
         if (bk_tl_mid_emit(c->q, &t) || bk_sync(c->q)) TL_FAIL();
@@ -220,20 +193,19 @@ int flbgpu_lines_to_events_parsed(flbgpu_parser *p, const char *text, size_t byt
         t.n_rec = (uint32_t) c->st.records_in;
         t.r_off = c->d_off; t.r_len = c->d_len; t.r_kind = c->d_kind; t.r_size = c->d_size; t.r_bsum = c->d_bsum;
         t.res = c->d_out; t.prep = c->d_prep;
-        TL_GROW(c->d_tl_rec, c->cap_tl_rec, (size_t) t.n_rec + 1, uint32_t);
+        if (dev_grow(c, (void **) &c->d_tl_rec, &c->cap_tl_rec, (size_t) t.n_rec + 1, sizeof(uint32_t), 0)) TL_FAIL();
         t.r_out = c->d_tl_rec;
         if (bk_tl_sizes(c->q, &t)) TL_FAIL();
     }
     if (bk_d2h(c->q, &last_nl, e->nl + (e->n_lines - 1), sizeof(last_nl)) || bk_d2h(c->q, &n_events, e->n_events, sizeof(n_events)) ||
-        bk_d2h(c->q, &bad, t.bad, sizeof(bad)) || bk_sizes_scan(c->q, t.size, mid_total ? e->n_lines : 0, d_fbsum, c->h_tl_bsum)) TL_FAIL();
+        bk_d2h(c->q, &bad, t.bad, sizeof(bad)) ||
+        sizes_to_offsets(c, t.size, mid_total ? e->n_lines : 0, d_fbsum, c->h_tl_bsum, "result larger than 4 GiB", &total)) TL_FAIL();
     if (bad) { set_err("parser call: the lines did not come back one to one%s%s", NULL, NULL); TL_FAIL(); }
-    total = mid_total ? c->h_tl_bsum[nbl] : 0;
-    if (total >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); TL_FAIL(); }
     if (consumed) *consumed = (size_t) last_nl + 1;
     if (lines) *lines = (size_t) n_events;
     if (total) {
         void *out;
-        TL_GROW(c->d_tl_out, c->cap_tl_out, total, uint8_t);
+        if (dev_grow(c, (void **) &c->d_tl_out, &c->cap_tl_out, total, 1, 0)) TL_FAIL();
         out = malloc((size_t) total);
         if (!out) { set_err("out of memory%s%s", NULL, NULL); TL_FAIL(); }
         if (bk_tl_emit(c->q, &t, d_fbsum, c->d_tl_out) || bk_d2h(c->q, out, c->d_tl_out, (size_t) total) || bk_sync(c->q)) { free(out); TL_FAIL(); }
@@ -242,6 +214,5 @@ int flbgpu_lines_to_events_parsed(flbgpu_parser *p, const char *text, size_t byt
     c->st.bytes_in = bytes; c->st.bytes_out = total; c->st.kernel_launches = bk_launch_count();
     pthread_mutex_unlock(&c->lock);
     return 0;
-#undef TL_GROW
 #undef TL_FAIL
 }

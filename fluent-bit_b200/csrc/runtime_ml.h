@@ -262,8 +262,8 @@ static int ml_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_ext,
     const struct cf_ml *cf = (const struct cf_ml *) (c->blob.p + c->ml_cfg_off);
     const uint8_t *d_in;
     struct ml_env e;
-    uint32_t n_rec = 0, n_ev, nb, h_flags[FLBGPU_MAX_FILTERS + 1];
-    size_t off = 0, S = slice_bytes(), need, at;
+    uint32_t n_rec, n_ev, h_flags[FLBGPU_MAX_FILTERS + 1];
+    size_t off, need, at;
     unsigned long long res[4];
     uint64_t total;
     struct timespec now;
@@ -274,33 +274,11 @@ static int ml_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_ext,
     if (bytes >= 0xfff00000ull) { set_err("chunk larger than 4 GiB: split the append%s%s", NULL, NULL); return -1; }
     if (d_in_ext) { d_in = d_in_ext; bk_upload_none(c->q); }
     else {
-        GROW(c->d_in, c->cap_in, bytes + 64, uint8_t);
+        if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0)) return -1;
         d_in = c->d_in;
         if (bk_upload_start(c->q, c->d_in, h_in, bytes)) return -1;
     }
-    if (bk_flags_clear(c->q, c->d_flags)) return -1;
-    /* ---- record index, slice by slice ---- */
-    while (off < bytes) {
-        size_t len = bytes - off < S ? bytes - off : S;
-        uint32_t n_tiles = (uint32_t) ((len + ((uintptr_t) (d_in + off) & 15) + BK_INDEX_TILE - 1) / BK_INDEX_TILE), n_cand = 0, n_valid = 0;
-        uint64_t end_off = off;
-        int tiled = 0;
-        if (bk_upload_wait_index(c->q, off + len)) return -1;
-        GROW(c->d_tile, c->cap_tile, n_tiles + 1, uint32_t);
-        if (bk_index_count(c->q, d_in, off, (uint32_t) len, c->d_tile, n_tiles, &n_cand)) return -1;
-        if (ensure_rec_cap(c, (size_t) n_rec + n_cand, n_rec)) return -1;
-        if (bk_index_fill(c->q, d_in, off, (uint32_t) len, c->d_tile, n_tiles, n_cand, c->d_off + n_rec, c->d_len + n_rec,
-                          c->d_kind + n_rec, &n_valid, &end_off, &tiled)) {
-            c->st.error_bits = FLBGPU_E_INDEX;
-            return -1;
-        }
-        if (n_valid == 0) {
-            if (off + len < bytes) { S *= 2; continue; }
-            break;
-        }
-        n_rec += n_valid;
-        off = (size_t) end_off;
-    }
+    if (bk_flags_clear(c->q, c->d_flags) || index_chunk(c, d_in, bytes, &n_rec, &off)) return -1;
     REFUSE_WIDE_ARRAYS(h_in, d_in, return -1);
     c->st.records_in = n_rec;
     c->st.passes = 1;
@@ -340,7 +318,7 @@ static int ml_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_ext,
             ML_CARVE(ev_ctx, uint32_t, 2 * (size_t) n_rec + 2);
             if (round == 0) {
                 need = at + 64;
-                GROW(c->d_mlw, c->cap_mlw, need, uint8_t);
+                if (dev_grow(c, (void **) &c->d_mlw, &c->cap_mlw, need, 1, 0)) return -1;
                 base = c->d_mlw;
             }
         }
@@ -357,19 +335,9 @@ static int ml_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_ext,
         return FLBGPU_FILTER_NOTOUCH;
     }
     /* ---- sizes, offsets ---- */
-    nb = (n_ev + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
-    GROW(c->d_bsum, c->cap_bsum, nb + 2, uint64_t);
-    if (c->cap_hbsum < (size_t) nb + 2) {
-        free(c->h_bsum);
-        c->cap_hbsum = (size_t) nb + nb / 4 + 64;
-        c->h_bsum = malloc(c->cap_hbsum * sizeof(uint64_t));
-        if (!c->h_bsum) { c->cap_hbsum = 0; return -1; }
-    }
-    if (bk_ml_sizes(c->q, &e, n_ev) || bk_sizes_scan(c->q, e.ev_size, n_ev, c->d_bsum, c->h_bsum)) return -1;
-    if (bk_flags_fetch(c->q, c->d_flags, h_flags)) return -1;
+    if (bk_ml_sizes(c->q, &e, n_ev) || bk_flags_fetch(c->q, c->d_flags, h_flags)) return -1;
     if (refused(c, h_flags[FLBGPU_MAX_FILTERS])) return -1;
-    total = c->h_bsum[nb];
-    if (total >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); return -1; }
+    if (sizes_to_offsets(c, e.ev_size, n_ev, NULL, NULL, "result larger than 4 GiB", &total)) return -1;
     c->st.bytes_out = total;
     c->st.records_out = n_ev;
     *out_size = (size_t) total;
@@ -378,8 +346,7 @@ static int ml_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_ext,
     if (total == 0) return FLBGPU_FILTER_NOTOUCH;
     /* ---- emit ---- */
     if (!host_out && !ext_out) {                         /* the result stays in this chain's own device buffer (ml_then_rest) */
-        GROW(c->d_out, c->cap_out, total, uint8_t);
-        if (bk_ml_emit(c->q, &e, n_ev, c->d_bsum, c->d_out) || bk_sync(c->q)) return -1;
+        if (dev_grow(c, (void **) &c->d_out, &c->cap_out, total, 1, 0) || bk_ml_emit(c->q, &e, n_ev, c->d_bsum, c->d_out) || bk_sync(c->q)) return -1;
     }
     else if (!host_out) {
         if (ext_cap < total) { set_err("device output buffer too small%s%s", NULL, NULL); return -1; }
@@ -388,8 +355,7 @@ static int ml_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_ext,
     else {
         void *out = malloc((size_t) total);
         if (!out) return -1;
-        GROW(c->d_out, c->cap_out, total, uint8_t);
-        if (bk_ml_emit(c->q, &e, n_ev, c->d_bsum, c->d_out) || bk_d2h(c->q, out, c->d_out, (size_t) total) || bk_sync(c->q)) { free(out); return -1; }
+        if (dev_grow(c, (void **) &c->d_out, &c->cap_out, total, 1, 0) || bk_ml_emit(c->q, &e, n_ev, c->d_bsum, c->d_out) || bk_d2h(c->q, out, c->d_out, (size_t) total) || bk_sync(c->q)) { free(out); return -1; }
         *host_out = out;
     }
     c->st.kernel_launches = bk_launch_count();

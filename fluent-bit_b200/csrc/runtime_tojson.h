@@ -22,12 +22,13 @@ static int tj_run(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, int json_f
 {
     struct tj_env e;
     const uint8_t *d_in;
-    uint32_t n_rec = 0, nb, h_flags[FLBGPU_MAX_FILTERS + 1];
-    size_t off = 0, S = slice_bytes(), at, need;
+    uint32_t n_rec, h_flags[FLBGPU_MAX_FILTERS + 1];
+    size_t off, at, need;
     unsigned long long undef = 0, cnt[2] = { 0, 0 };
     uint32_t *d_groups = NULL;
     uint64_t total;
     char *res;
+    int pass;
 
     memset(&c->st, 0, sizeof(c->st));
     c->st.bytes_in = bytes;
@@ -42,35 +43,13 @@ static int tj_run(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, int json_f
     }
     e.json_format = (uint32_t) json_format; e.date_format = (uint32_t) date_format; e.escape_unicode = escape_unicode ? 1u : 0u;
     if (bytes) {
-        GROW(c->d_in, c->cap_in, bytes + 64, uint8_t);
+        if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0)) return -1;
         if (bk_upload_start(c->q, c->d_in, h_in, bytes)) return -1;
     }
     d_in = c->d_in;
-    if (bk_flags_clear(c->q, c->d_flags)) return -1;
-    while (off < bytes) {                              /* record index, slice by slice */
-        size_t len = bytes - off < S ? bytes - off : S;
-        uint32_t n_tiles = (uint32_t) ((len + ((uintptr_t) (d_in + off) & 15) + BK_INDEX_TILE - 1) / BK_INDEX_TILE), n_cand = 0, n_valid = 0;
-        uint64_t end_off = off;
-        int tiled = 0;
-        if (bk_upload_wait_index(c->q, off + len)) return -1;
-        GROW(c->d_tile, c->cap_tile, n_tiles + 1, uint32_t);
-        if (bk_index_count(c->q, d_in, off, (uint32_t) len, c->d_tile, n_tiles, &n_cand)) return -1;
-        if (ensure_rec_cap(c, (size_t) n_rec + n_cand, n_rec)) return -1;
-        if (bk_index_fill(c->q, d_in, off, (uint32_t) len, c->d_tile, n_tiles, n_cand, c->d_off + n_rec, c->d_len + n_rec,
-                          c->d_kind + n_rec, &n_valid, &end_off, &tiled)) {
-            c->st.error_bits = FLBGPU_E_INDEX;
-            return -1;
-        }
-        if (n_valid == 0) {
-            if (off + len < bytes) { S *= 2; continue; }
-            break;
-        }
-        n_rec += n_valid;
-        off = (size_t) end_off;
-    }
+    if (bk_flags_clear(c->q, c->d_flags) || index_chunk(c, d_in, bytes, &n_rec, &off)) return -1;
     REFUSE_WIDE_ARRAYS(h_in, d_in, return -1);
     c->st.records_in = n_rec;
-    nb = (n_rec + BK_REC_BLOCK - 1) / BK_REC_BLOCK;
     total = 0;
     if (n_rec) {
         e.in = d_in; e.off = c->d_off; e.len = c->d_len; e.kind = c->d_kind; e.n_rec = n_rec;
@@ -80,56 +59,40 @@ static int tj_run(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, int json_f
         /* work memory: the counters (undefined strings, group markers), the marker lists, the packed lengths, the scratch slices */
         e.marks_cap = TJ_MARKS_CAP;
         need = 16 + 3 * sizeof(uint32_t) * (size_t) TJ_MARKS_CAP + sizeof(uint32_t) * (size_t) n_rec + 64;
-        GROW(c->d_mlw, c->cap_mlw, need, uint8_t);
+        if (dev_grow(c, (void **) &c->d_mlw, &c->cap_mlw, need, 1, 0)) return -1;
         at = 0;
         e.undefined = (unsigned long long *) (c->d_mlw + at); e.n_marks = e.undefined + 1; at += 16;
         e.marks = (uint32_t *) (c->d_mlw + at); at += 2 * sizeof(uint32_t) * (size_t) TJ_MARKS_CAP;
         d_groups = (uint32_t *) (c->d_mlw + at); at += sizeof(uint32_t) * (size_t) TJ_MARKS_CAP;
         e.plen = (uint32_t *) (c->d_mlw + at);
-        GROW(c->d_scr, c->cap_scr, bytes + (size_t) n_rec * e.scr_pad + 64, uint8_t);
-        e.scr = c->d_scr;
-        if (bk_zero(c->q, e.undefined, 16)) return -1;
-        GROW(c->d_bsum, c->cap_bsum, nb + 2, uint64_t);
-        if (c->cap_hbsum < (size_t) nb + 2) {
-            free(c->h_bsum);
-            c->cap_hbsum = (size_t) nb + nb / 4 + 64;
-            c->h_bsum = malloc(c->cap_hbsum * sizeof(uint64_t));
-            if (!c->h_bsum) { c->cap_hbsum = 0; return -1; }
-        }
-        if (bk_tj_sizes(c->q, &e) || bk_sizes_scan(c->q, c->d_size, n_rec, c->d_bsum, c->h_bsum)) return -1;
-        if (bk_flags_fetch(c->q, c->d_flags, h_flags)) return -1;
-        if (h_flags[FLBGPU_MAX_FILTERS] & FLBGPU_E_JSONDATE) return 1;          /* the reference returns NULL for such a chunk */
-        if (refused(c, h_flags[FLBGPU_MAX_FILTERS])) return -1;
-        total = c->h_bsum[nb];
-        if (total >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); return -1; }
-        if (bk_d2h(c->q, cnt, e.undefined, sizeof(cnt)) || bk_sync(c->q)) return -1;
-        if (cnt[1]) {
-            /* group markers in the chunk: the events behind a start carry its body as group_attributes -- the list in record
-             * order, and the sizing pass again with it */
-            uint32_t *h = malloc(2 * sizeof(uint32_t) * (size_t) cnt[1]), maxlen = 0;
-            size_t a, b2;
-            if (!h) return -1;
-            if (bk_d2h(c->q, h, e.marks, 2 * sizeof(uint32_t) * (size_t) cnt[1]) || bk_sync(c->q)) { free(h); return -1; }
-            for (a = 0; a < (size_t) cnt[1]; a++) { if (h[2 * a + 1] > maxlen) maxlen = h[2 * a + 1]; h[a] = h[2 * a]; }
-            for (a = 1; a < (size_t) cnt[1]; a++) {      /* a handful: insertion sort */
-                const uint32_t v = h[a];
-                for (b2 = a; b2 > 0 && h[b2 - 1] > v; b2--) h[b2] = h[b2 - 1];
-                h[b2] = v;
-            }
-            if (bk_h2d(c->q, d_groups, h, sizeof(uint32_t) * (size_t) cnt[1]) || bk_sync(c->q)) { free(h); return -1; }
-            free(h);
-            e.groups = d_groups; e.n_groups = (uint32_t) cnt[1];
-            e.scr_pad += maxlen + 32;                   /* an event's packed map now holds a marker's body too */
-            GROW(c->d_scr, c->cap_scr, bytes + (size_t) n_rec * e.scr_pad + 64, uint8_t);
+        /* sized once, and once more when the chunk holds group markers: the events behind a start carry its body as
+         * group_attributes */
+        for (pass = 0; ; pass++) {
+            if (dev_grow(c, (void **) &c->d_scr, &c->cap_scr, bytes + (size_t) n_rec * e.scr_pad + 64, 1, 0)) return -1;
             e.scr = c->d_scr;
-            if (bk_zero(c->q, e.undefined, 8)) return -1;
-            if (bk_tj_sizes(c->q, &e) || bk_sizes_scan(c->q, c->d_size, n_rec, c->d_bsum, c->h_bsum)) return -1;
-            if (bk_flags_fetch(c->q, c->d_flags, h_flags)) return -1;
-            if (h_flags[FLBGPU_MAX_FILTERS] & FLBGPU_E_JSONDATE) return 1;
+            if (bk_zero(c->q, e.undefined, pass ? 8 : 16) || bk_tj_sizes(c->q, &e) || bk_flags_fetch(c->q, c->d_flags, h_flags)) return -1;
+            if (h_flags[FLBGPU_MAX_FILTERS] & FLBGPU_E_JSONDATE) return 1;          /* the reference returns NULL for such a chunk */
             if (refused(c, h_flags[FLBGPU_MAX_FILTERS])) return -1;
-            total = c->h_bsum[nb];
-            if (total >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); return -1; }
+            if (sizes_to_offsets(c, c->d_size, n_rec, NULL, NULL, "result larger than 4 GiB", &total)) return -1;
             if (bk_d2h(c->q, cnt, e.undefined, sizeof(cnt)) || bk_sync(c->q)) return -1;
+            if (pass || !cnt[1]) break;
+            {
+                /* the markers' list in record order */
+                uint32_t *h = malloc(2 * sizeof(uint32_t) * (size_t) cnt[1]), maxlen = 0;
+                size_t a, b2;
+                if (!h) return -1;
+                if (bk_d2h(c->q, h, e.marks, 2 * sizeof(uint32_t) * (size_t) cnt[1]) || bk_sync(c->q)) { free(h); return -1; }
+                for (a = 0; a < (size_t) cnt[1]; a++) { if (h[2 * a + 1] > maxlen) maxlen = h[2 * a + 1]; h[a] = h[2 * a]; }
+                for (a = 1; a < (size_t) cnt[1]; a++) {      /* a handful: insertion sort */
+                    const uint32_t v = h[a];
+                    for (b2 = a; b2 > 0 && h[b2 - 1] > v; b2--) h[b2] = h[b2 - 1];
+                    h[b2] = v;
+                }
+                if (bk_h2d(c->q, d_groups, h, sizeof(uint32_t) * (size_t) cnt[1]) || bk_sync(c->q)) { free(h); return -1; }
+                free(h);
+                e.groups = d_groups; e.n_groups = (uint32_t) cnt[1];
+                e.scr_pad += maxlen + 32;                   /* an event's packed map now holds a marker's body too */
+            }
         }
         undef = cnt[0];
     }
@@ -141,8 +104,7 @@ static int tj_run(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, int json_f
         res = malloc((size_t) total + 3);
         if (!res) return -1;
         if (total) {
-            GROW(c->d_out, c->cap_out, total, uint8_t);
-            if (bk_tj_emit(c->q, &e, c->d_bsum, c->d_out) || bk_d2h(c->q, res, c->d_out, (size_t) total) || bk_sync(c->q)) { free(res); return -1; }
+            if (dev_grow(c, (void **) &c->d_out, &c->cap_out, total, 1, 0) || bk_tj_emit(c->q, &e, c->d_bsum, c->d_out) || bk_d2h(c->q, res, c->d_out, (size_t) total) || bk_sync(c->q)) { free(res); return -1; }
             res[0] = '[';
             res[total] = ']'; res[total + 1] = 0;
             *out_size = (size_t) total + 1;
@@ -154,8 +116,7 @@ static int tj_run(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, int json_f
     if (total == 0) return 1;
     res = malloc((size_t) total + 1);
     if (!res) return -1;
-    GROW(c->d_out, c->cap_out, total, uint8_t);
-    if (bk_tj_emit(c->q, &e, c->d_bsum, c->d_out) || bk_d2h(c->q, res, c->d_out, (size_t) total) || bk_sync(c->q)) { free(res); return -1; }
+    if (dev_grow(c, (void **) &c->d_out, &c->cap_out, total, 1, 0) || bk_tj_emit(c->q, &e, c->d_bsum, c->d_out) || bk_d2h(c->q, res, c->d_out, (size_t) total) || bk_sync(c->q)) { free(res); return -1; }
     res[total] = 0;
     *out = res; *out_size = (size_t) total;
     c->st.bytes_out = total;
