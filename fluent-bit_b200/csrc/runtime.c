@@ -1958,25 +1958,56 @@ static int ends_cleanly(bk_q *q, const uint8_t *h_in, const uint8_t *d_in, size_
 
 /* The record index frames events whose root and header arrays are fixarrays (0x92), which is all msgpack-c's
  * packer ever writes for two elements.  The reference's decoder would also take the same arrays spelled as
- * array16 / array32: when the decodable prefix stops at such a spelling the call is refused, not cut short. */
-static int stops_at_wide_array(bk_q *q, const uint8_t *h_in, const uint8_t *d_in, size_t off, size_t bytes)
+ * array16 / array32: when the decodable prefix [0, off) stops at such a spelling the call is refused, not cut short.
+ * Nonzero = refused (FLBGPU_E_INDEX and the error text are set). */
+static int refuse_wide_arrays(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in, size_t off, size_t bytes)
 {
     uint8_t b[8] = { 0 };
     size_t n = bytes - off < sizeof(b) ? bytes - off : sizeof(b), i = 0;
+    int wide = 0;
     if (n == 0) return 0;
     if (h_in) memcpy(b, h_in + off, n);
-    else if (bk_d2h(q, b, d_in + off, n) || bk_sync(q)) return 0;
+    else if (bk_d2h(c->q, b, d_in + off, n) || bk_sync(c->q)) return 0;
     if (b[0] == 0x92) i = 1;                                   /* [ [ts, meta], body ] with a wide header array */
-    if (b[i] == 0xdc) return b[i + 1] == 0 && b[i + 2] == 2;
-    if (b[i] == 0xdd) return b[i + 1] == 0 && b[i + 2] == 0 && b[i + 3] == 0 && b[i + 4] == 2;
+    if (b[i] == 0xdc) wide = b[i + 1] == 0 && b[i + 2] == 2;
+    if (b[i] == 0xdd) wide = b[i + 1] == 0 && b[i + 2] == 0 && b[i + 3] == 0 && b[i + 4] == 2;
+    if (!wide) return 0;
+    c->st.error_bits = FLBGPU_E_INDEX;
+    snprintf(g_rt_err, sizeof(g_rt_err), "event framed with an array16/array32 header at byte %zu: not decoded on the GPU path", off);
+    return 1;
+}
+
+/* the start of a chain call: fresh stats, no result yet, the call's clock (t0, when given) running.  A chunk of 4 GiB or
+ * more is refused: record offsets are 32-bit. */
+static int call_start(flbgpu_chain *c, size_t bytes, size_t *out_size, struct timespec *t0)
+{
+    memset(&c->st, 0, sizeof(c->st));
+    c->st.bytes_in = bytes;
+    *out_size = 0;
+    if (t0) clock_gettime(CLOCK_MONOTONIC, t0);
+    if (bytes >= 0xfff00000ull) { set_err("chunk larger than 4 GiB: split the append%s%s", NULL, NULL); return -1; }
     return 0;
 }
-#define REFUSE_WIDE_ARRAYS(h_in_, d_in_, fail_stmt) do { \
-        if (off < bytes && stops_at_wide_array(c->q, h_in_, d_in_, off, bytes)) { \
-            c->st.error_bits = FLBGPU_E_INDEX; \
-            snprintf(g_rt_err, sizeof(g_rt_err), "event framed with an array16/array32 header at byte %zu: not decoded on the GPU path", off); \
-            fail_stmt; \
-        } } while (0)
+
+/* the chunk on the device: h_in uploaded in pieces into the chain's input buffer (the index waits for each piece), or the
+ * caller's d_in_ext as it is.  NULL on failure. */
+static const uint8_t *place_input(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_ext, size_t bytes)
+{
+    if (d_in_ext) { bk_upload_none(c->q); return d_in_ext; }
+    if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0) || bk_upload_start(c->q, c->d_in, h_in, bytes)) return NULL;
+    return c->d_in;
+}
+
+/* the scratch a call needs, its arguments before the first evaluation (fill_args() adds the buffers once they have grown)
+ * and the per-call evidence, metrics and parser report cleared */
+static int call_args(flbgpu_chain *c, struct bk_chain_args *a, size_t bytes, uint32_t assume)
+{
+    if (c->needs_scratch && dev_grow(c, (void **) &c->d_scr, &c->cap_scr, (size_t) c->scr_mul * bytes + 64, 1, 0)) return -1;
+    memset(a, 0, sizeof(*a));
+    a->now = (int64_t) time(NULL);
+    a->assume = assume;
+    return (bk_flags_clear(c->q, c->d_flags) || l2m_clear(c) || report_clear(c)) ? -1 : 0;
+}
 
 #include "runtime_ml.h"
 #include "runtime_tojson.h"
@@ -2029,6 +2060,12 @@ static uint32_t initial_assume(flbgpu_chain *c)
     uint32_t a = c->active;
     if (c->l2m_index >= 0 && !c->f[c->l2m_index]->l2m->discard) a &= ~(1u << c->l2m_index);
     return a;
+}
+
+/* the verdict vector the speculating forms emit under: the one the previous call settled on, if it had the same routing */
+static uint32_t speculated_assume(flbgpu_chain *c)
+{
+    return (c->spec_valid && c->spec_active == c->active) ? c->spec_assume : initial_assume(c);
 }
 
 /* One call.  Input: h_in (host, uploaded in pieces) or d_in_ext (already in HBM).
@@ -2099,6 +2136,17 @@ static int rtag_collect(flbgpu_chain *c, const struct bk_chain_args *a, uint32_t
     return 0;
 }
 
+/* What a call leaves behind once no other form will redo it: its metrics folded into the filter's table and, with a
+ * routed rewrite_tag filter, the re-tagged stream of its n_rec records.  Those go to the emitter whatever the filter's own
+ * verdict is (a chunk that does not decode to its end makes it NOTOUCH after the fact, rewrite_tag.c:500-546). */
+static int call_commit(flbgpu_chain *c, struct bk_chain_args *a, const uint8_t *d_in, size_t bytes, uint32_t n_rec, const uint32_t *flags)
+{
+    if (l2m_merge(c)) return -1;
+    if (c->rtag_index < 0 || !((c->active >> c->rtag_index) & 1)) return 0;
+    fill_args(c, a, d_in, bytes, n_rec);
+    return rtag_collect(c, a, n_rec, (flags[c->rtag_index] & CHF_CAUSE) != 0);
+}
+
 /* the host buffer a result of `need` bytes goes to: the caller's (flbgpu_chain_set_result_buffer) while it fits, else a
  * malloc() of `size` bytes; res_drop() releases it on failure */
 static void *res_take(flbgpu_chain *c, size_t need, size_t size)
@@ -2143,22 +2191,8 @@ static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_e
     int clean, pass;
     struct timespec t0;
 
-    memset(&c->st, 0, sizeof(c->st));
-    c->st.bytes_in = bytes;
-    *out_size = 0;
-    clock_gettime(CLOCK_MONOTONIC, &t0);
-    if (bytes >= 0xfff00000ull) { set_err("chunk larger than 4 GiB: split the append%s%s", NULL, NULL); return -1; }
-    if (d_in_ext) { d_in = d_in_ext; bk_upload_none(c->q); }
-    else {
-        if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0)) return -1;
-        d_in = c->d_in;
-        if (bk_upload_start(c->q, c->d_in, h_in, bytes)) return -1;
-    }
-    if (c->needs_scratch && dev_grow(c, (void **) &c->d_scr, &c->cap_scr, (size_t) c->scr_mul * bytes + 64, 1, 0)) return -1;
-    memset(&a, 0, sizeof(a));
-    a.now = (int64_t) time(NULL);
-    a.assume = initial_assume(c);
-    if (bk_flags_clear(c->q, c->d_flags) || l2m_clear(c) || report_clear(c)) return -1;
+    if (call_start(c, bytes, out_size, &t0) || !(d_in = place_input(c, h_in, d_in_ext, bytes)) ||
+        call_args(c, &a, bytes, initial_assume(c))) return -1;
 
     /* ---- index + evaluate, slice by slice, while the upload is still running ---- */
     while (off < bytes) {
@@ -2177,7 +2211,7 @@ static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_e
         off = (size_t) end_off;
     }
     clean = ends_cleanly(c->q, h_in, d_in, off, bytes);
-    REFUSE_WIDE_ARRAYS(h_in, d_in, return -1);
+    if (refuse_wide_arrays(c, h_in, d_in, off, bytes)) return -1;
     c->st.records_in = n_rec;
     c->st.passes = 1;
     fill_args(c, &a, d_in, bytes, n_rec);
@@ -2193,10 +2227,7 @@ static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_e
     }
     c->st.kernel_launches = bk_launch_count();
     c->st.phase_ms[0] = ms_since(&t0);
-    if (l2m_merge(c)) return -1;
-    /* the records a rewrite_tag filter matched go to its emitter whatever the filter's own verdict is (a chunk that does not
-     * decode to its end makes it NOTOUCH after the fact, rewrite_tag.c:500-546) */
-    if (a.d_esize && rtag_collect(c, &a, n_rec, (h_flags[c->rtag_index] & CHF_CAUSE) != 0)) return -1;
+    if (call_commit(c, &a, d_in, bytes, n_rec, h_flags)) return -1;
     if (a.assume == 0) return FLBGPU_FILTER_NOTOUCH;
 
     /* ---- output offsets ---- */
@@ -2276,6 +2307,53 @@ void flbgpu_stream_copy(void *dst, const void *src, size_t n)
     memcpy(dst, src, n);
 }
 
+/* The streaming form's result so far: the host buffer and its capacity, the bytes placed in it, the record blocks emitted,
+ * and whether a download into it is open. */
+struct stream_out { uint8_t *out; size_t cap_out_h; uint64_t placed; uint32_t b_done; int dl_open; };
+
+/* Emit the record blocks [so->b_done, upto) of the n_rec records evaluated so far (input bytes [0, off)) behind what has
+ * been placed, and send them to the host buffer, which grows with the result. */
+static int stream_flush(flbgpu_chain *c, struct bk_chain_args *a, struct stream_out *so, uint32_t upto, uint32_t n_rec, size_t off, size_t bytes)
+{
+    uint64_t end;
+    if (upto <= so->b_done) return 0;
+    fill_args(c, a, c->d_in, bytes, n_rec);
+    if (bk_sizes_scan_range(c->q, c->d_size, n_rec, so->b_done, upto, c->d_bsum, c->h_bsum, so->placed)) return -1;
+    end = c->h_bsum[upto];
+    if (end >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); return -1; }
+    if (end > so->placed) {
+        if (end > so->cap_out_h) {
+            /* first estimate from the output/input ratio so far; grown (rarely) when it was too low */
+            double ratio = (double) end / (double) (off ? off : 1);
+            size_t want = (size_t) (ratio * 1.15 * (double) bytes) + ((size_t) 8 << 20);
+            uint8_t *no;
+            if (want < end) want = (size_t) end + ((size_t) 8 << 20);
+            if (so->dl_open) { so->dl_open = 0; if (bk_download_end(c->q)) return -1; }
+            if (!so->out) no = res_take(c, (size_t) end, want);
+            else if (so->out == c->res_buf) { no = malloc(want); if (no) memcpy(no, so->out, (size_t) so->placed); }     /* outgrown: what has arrived moves */
+            else no = realloc(so->out, want);
+            if (!no) return -1;
+            if (no == c->res_buf) want = c->res_cap;
+            so->out = no; so->cap_out_h = want;
+            if (so->out != c->res_buf) hugepage_hint(so->out, want);
+            /* the device output buffer grows with the host one; bytes already emitted stay where they are */
+            if (dev_grow(c, (void **) &c->d_out, &c->cap_out, want, 1, (size_t) so->placed)) return -1;
+        }
+        if (!so->dl_open) { if (bk_download_begin(c->q, so->out, c->d_out)) return -1; so->dl_open = 1; }
+        if (bk_chain_emit(c->q, a, c->d_out, so->b_done, upto) || bk_download_push(c->q, (size_t) so->placed, (size_t) end)) return -1;
+    }
+    so->placed = end;
+    so->b_done = upto;
+    return 0;
+}
+
+/* the streaming form gives its result up: the download closes, the buffer is released (the caller's stays the caller's) */
+static void stream_drop(flbgpu_chain *c, struct stream_out *so)
+{
+    if (so->dl_open) bk_download_end(c->q);
+    res_drop(c, so->out);
+}
+
 /* Streaming form of chain_run for host buffers.  The chunk-level verdicts are only known when the
  * whole chunk has been evaluated, but they almost never differ from the previous call's (and from
  * "every filter modifies" on the first call), so each slice is emitted and sent back as soon as it
@@ -2285,63 +2363,18 @@ void flbgpu_stream_copy(void *dst, const void *src, size_t n)
 static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, void **host_out, size_t *out_size, int *ret)
 {
     struct bk_chain_args a;
-    uint32_t n_rec = 0, h_flags[FLBGPU_MAX_FILTERS + 1], b_done = 0, assume, nb_max;
-    size_t off = 0, S = slice_bytes(), cap_out_h = 0, force = 0;
+    struct stream_out so = { NULL, 0, 0, 0, 0 };
+    uint32_t n_rec = 0, h_flags[FLBGPU_MAX_FILTERS + 1], assume = speculated_assume(c), nb_max;
+    size_t off = 0, S = slice_bytes(), force = 0;
     const int taper = !(getenv("FLBGPU_TAPER") && getenv("FLBGPU_TAPER")[0] == '0');
-    uint64_t placed = 0;
-    uint8_t *out = NULL;
-    int clean, dl_open = 0;
+    int clean;
     struct timespec t0;
 
-    memset(&c->st, 0, sizeof(c->st));
-    c->st.bytes_in = bytes;
-    *out_size = 0;
-    clock_gettime(CLOCK_MONOTONIC, &t0);
-    assume = initial_assume(c);
-    if (c->spec_valid && c->spec_active == c->active) assume = c->spec_assume;
     if (assume == 0) return 1;                       /* nothing would be emitted: the classic path decides */
-    if (bytes >= 0xfff00000ull) { set_err("chunk larger than 4 GiB: split the append%s%s", NULL, NULL); return -1; }
-    if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0)) return -1;
-    if (bk_upload_start(c->q, c->d_in, h_in, bytes)) return -1;
-    if (c->needs_scratch && dev_grow(c, (void **) &c->d_scr, &c->cap_scr, (size_t) c->scr_mul * bytes + 64, 1, 0)) return -1;
+    if (call_start(c, bytes, out_size, &t0) || !place_input(c, h_in, NULL, bytes)) return -1;
     nb_max = (uint32_t) (bytes / (3 * BK_REC_BLOCK)) + 4;       /* an event is at least 3 bytes */
     if (dev_grow(c, (void **) &c->d_bsum, &c->cap_bsum, nb_max, sizeof(uint64_t), 0) ||
-        host_grow((void **) &c->h_bsum, &c->cap_hbsum, nb_max, sizeof(uint64_t))) return -1;
-    memset(&a, 0, sizeof(a));
-    a.now = (int64_t) time(NULL);
-    a.assume = assume;
-    if (bk_flags_clear(c->q, c->d_flags) || l2m_clear(c) || report_clear(c)) return -1;
-
-#define STREAM_FLUSH(upto_blocks) do { \
-        uint32_t b1_ = (upto_blocks); \
-        if (b1_ > b_done) { \
-            fill_args(c, &a, c->d_in, bytes, n_rec); \
-            if (bk_sizes_scan_range(c->q, c->d_size, n_rec, b_done, b1_, c->d_bsum, c->h_bsum, placed)) goto fail; \
-            if (c->h_bsum[b1_] >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); goto fail; } \
-            if (c->h_bsum[b1_] > placed) { \
-                if (c->h_bsum[b1_] > cap_out_h) { \
-                    /* first estimate from the output/input ratio so far; grown (rarely) when it was too low */ \
-                    double ratio_ = (double) c->h_bsum[b1_] / (double) (off ? off : 1); \
-                    size_t want_ = (size_t) (ratio_ * 1.15 * (double) bytes) + ((size_t) 8 << 20); \
-                    uint8_t *no_; \
-                    if (want_ < c->h_bsum[b1_]) want_ = (size_t) c->h_bsum[b1_] + ((size_t) 8 << 20); \
-                    if (dl_open) { if (bk_download_end(c->q)) { dl_open = 0; goto fail; } dl_open = 0; } \
-                    if (!out) no_ = res_take(c, (size_t) c->h_bsum[b1_], want_); \
-                    else if (out == c->res_buf) { no_ = malloc(want_); if (no_) memcpy(no_, out, (size_t) placed); }           /* outgrown: what has arrived moves */ \
-                    else no_ = realloc(out, want_); \
-                    if (!no_) goto fail; \
-                    if (no_ == c->res_buf) want_ = c->res_cap; \
-                    out = no_; cap_out_h = want_; \
-                    if (out != c->res_buf) hugepage_hint(out, want_); \
-                    /* the device output buffer grows with the host one; bytes already emitted stay where they are */ \
-                    if (dev_grow(c, (void **) &c->d_out, &c->cap_out, want_, 1, (size_t) placed)) goto fail; \
-                } \
-                if (!dl_open) { if (bk_download_begin(c->q, out, c->d_out)) goto fail; dl_open = 1; } \
-                if (bk_chain_emit(c->q, &a, c->d_out, b_done, b1_) || bk_download_push(c->q, (size_t) placed, (size_t) c->h_bsum[b1_])) goto fail; \
-            } \
-            placed = c->h_bsum[b1_]; \
-            b_done = b1_; \
-        } } while (0)
+        host_grow((void **) &c->h_bsum, &c->cap_hbsum, nb_max, sizeof(uint64_t)) || call_args(c, &a, bytes, assume)) return -1;
 
     while (off < bytes) {
         /* slices shrink towards the end of the chunk: what is left to do after the last upload piece
@@ -2359,7 +2392,7 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
         }
         force = 0;
         /* the previous slice has been evaluated by now (or is about to finish): place and send it */
-        STREAM_FLUSH(n_rec / BK_REC_BLOCK);
+        if (stream_flush(c, &a, &so, n_rec / BK_REC_BLOCK, n_rec, off, bytes)) goto fail;
         fill_args(c, &a, c->d_in, bytes, n_rec + n_valid);
         bk_hint_streaming(c->q, a.d_in + off, (size_t) end_off - off);
         if (bk_chain_eval(c->q, &a, n_rec, n_rec + n_valid)) goto fail;
@@ -2367,11 +2400,10 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
         off = (size_t) end_off;
     }
     clean = ends_cleanly(c->q, h_in, c->d_in, off, bytes);
-    REFUSE_WIDE_ARRAYS(h_in, c->d_in, goto fail);
+    if (refuse_wide_arrays(c, h_in, c->d_in, off, bytes)) goto fail;
     c->st.records_in = n_rec;
     c->st.passes = 1;
-    STREAM_FLUSH((n_rec + BK_REC_BLOCK - 1) / BK_REC_BLOCK);
-    c->st.phase_ms[0] = 0;
+    if (stream_flush(c, &a, &so, (n_rec + BK_REC_BLOCK - 1) / BK_REC_BLOCK, n_rec, off, bytes)) goto fail;
 
     /* ---- the verdicts must be the ones speculated on ---- */
     if (bk_flags_fetch(c->q, c->d_flags, h_flags)) goto fail;
@@ -2379,68 +2411,56 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
     if (settle(c, assume, h_flags, clean, &assume) >= 0) {
         /* evidence of the later filters was gathered under a wrong assumption: redo classically (the next call
          * speculates on the verdict as found) */
-        if (dl_open) bk_download_end(c->q);
-        res_drop(c, out);
+        stream_drop(c, &so);
         return 1;
     }
     c->st.kernel_launches = bk_launch_count();
-    if (l2m_merge(c)) goto fail;
-    if (dl_open) { dl_open = 0; if (bk_download_end(c->q)) goto fail; }
-    if (c->rtag_index >= 0 && ((c->active >> c->rtag_index) & 1)) {      /* every record of the call is still indexed: one re-tagged stream */
-        fill_args(c, &a, c->d_in, bytes, n_rec);
-        if (rtag_collect(c, &a, n_rec, (h_flags[c->rtag_index] & CHF_CAUSE) != 0)) goto fail;
-    }
+    if (so.dl_open) { so.dl_open = 0; if (bk_download_end(c->q)) goto fail; }
+    if (call_commit(c, &a, c->d_in, bytes, n_rec, h_flags)) goto fail;      /* every record of the call is still indexed */
     bk_records_out(c->q, &c->st.records_out);
-    c->st.bytes_out = placed;
-    *out_size = (size_t) placed;
-    if (placed == 0) { res_drop(c, out); out = NULL; }
-    else if (out != c->res_buf && cap_out_h > placed + placed / 2) {     /* badly over-estimated: give the excess back */
-        uint8_t *sh = realloc(out, (size_t) placed);
-        if (sh) out = sh;
+    c->st.bytes_out = so.placed;
+    *out_size = (size_t) so.placed;
+    if (so.placed == 0) { res_drop(c, so.out); so.out = NULL; }
+    else if (so.out != c->res_buf && so.cap_out_h > so.placed + so.placed / 2) {     /* badly over-estimated: give the excess back */
+        uint8_t *sh = realloc(so.out, (size_t) so.placed);
+        if (sh) so.out = sh;
     }
-    *host_out = out;
+    *host_out = so.out;
     c->st.phase_ms[3] = ms_since(&t0);
     *ret = FLBGPU_FILTER_MODIFIED;
     return 0;
 fail:
-    if (dl_open) bk_download_end(c->q);
-    res_drop(c, out);
+    stream_drop(c, &so);
     return -1;
-#undef STREAM_FLUSH
 }
 
-/* One append as flb_filter_do() hands it over (tens of KB to a few MB): the whole call is one stream of work
- * without a host synchronisation in between (bk_small_run), under the verdict vector the previous call settled
- * on.  Returns 0 (done, *ret set), 1 (not for this form or the speculation did not hold: use the general
- * paths), -1 error. */
+/* the largest append the small-chunk form takes */
 static size_t small_bytes(void)
 {
-    const char *e = getenv("FLBGPU_SMALL_MB"), *sv = getenv("FLBGPU_STREAM");
+    const char *e = getenv("FLBGPU_SMALL_MB");
     long mb = e ? atol(e) : 8;
     size_t v, s = slice_bytes();
-    if (sv && sv[0] == '0') return 0;                /* the classic two-pass form only */
     if (mb < 0) mb = 0;
     if (mb > 256) mb = 256;
     v = (size_t) mb << 20;
     return v < s ? v : s;                            /* the small form is a single slice */
 }
 
+/* One append as flb_filter_do() hands it over (tens of KB to a few MB): the whole call is one stream of work
+ * without a host synchronisation in between (bk_small_run), under the verdict vector the previous call settled
+ * on.  Returns 0 (done, *ret set), 1 (not for this form or the speculation did not hold: use the general
+ * paths), -1 error. */
 static int chain_run_small(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, void **host_out, size_t *out_size, int *ret)
 {
     struct bk_chain_args a;
     struct bk_small_res res;
-    uint32_t assume, n_tiles, cap_rec, nb_cap;
+    uint32_t assume = speculated_assume(c), n_tiles, cap_rec, nb_cap;
     size_t off, cap_out;
     int clean;
     struct timespec t0;
 
-    assume = initial_assume(c);
-    if (c->spec_valid && c->spec_active == c->active) assume = c->spec_assume;
     if (assume == 0) return 1;                       /* nothing would be emitted: the classic path decides */
-    memset(&c->st, 0, sizeof(c->st));
-    c->st.bytes_in = bytes;
-    *out_size = 0;
-    clock_gettime(CLOCK_MONOTONIC, &t0);
+    if (call_start(c, bytes, out_size, &t0)) return -1;
     /* records of the shapes this path serves are tens of bytes at least; a chunk of tinier events overflows
      * the arrays, which the device reports (res.overflow) and the general path then handles */
     cap_rec = (uint32_t) (bytes / 24) + 1024;
@@ -2449,16 +2469,15 @@ static int chain_run_small(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, v
     n_tiles = (uint32_t) ((bytes + BK_INDEX_TILE - 1) / BK_INDEX_TILE);
     cap_out = bytes + bytes / 2 + 4096;
     if (c->small_cap_out > cap_out) cap_out = c->small_cap_out;
+    /* (bk_small_run uploads the chunk itself, through the queue's own pinned buffer) */
     if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0) ||
-        (c->needs_scratch && dev_grow(c, (void **) &c->d_scr, &c->cap_scr, (size_t) c->scr_mul * bytes + 64, 1, 0)) ||
         dev_grow(c, (void **) &c->d_tile, &c->cap_tile, n_tiles + 1, sizeof(uint32_t), 0) ||
         dev_grow(c, (void **) &c->d_bsum, &c->cap_bsum, nb_cap + 2, sizeof(uint64_t), 0) ||
         ensure_rec_cap(c, cap_rec, 0) ||
-        dev_grow(c, (void **) &c->d_out, &c->cap_out, cap_out, 1, 0)) return -1;
+        dev_grow(c, (void **) &c->d_out, &c->cap_out, cap_out, 1, 0) ||
+        call_args(c, &a, bytes, assume)) return -1;
     cap_out = c->cap_out;
     fill_args(c, &a, c->d_in, bytes, 0);
-    a.assume = assume; a.now = (int64_t) time(NULL);
-    if (bk_flags_clear(c->q, c->d_flags) || l2m_clear(c) || report_clear(c)) return -1;
     if (bk_small_run(c->q, &a, h_in, c->d_in, bytes, cap_rec, c->d_tile, n_tiles, c->d_out, cap_out, &res)) return -1;
     c->st.kernel_launches = bk_launch_count();
     if (res.overflow) {                              /* denser events than assumed, or a slice-sized tangle of broken links */
@@ -2467,21 +2486,17 @@ static int chain_run_small(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, v
     }
     off = (size_t) res.end_off;
     clean = ends_cleanly(c->q, h_in, c->d_in, off, bytes);
-    REFUSE_WIDE_ARRAYS(h_in, c->d_in, return -1);
+    if (refuse_wide_arrays(c, h_in, c->d_in, off, bytes)) return -1;
     c->st.records_in = res.n_valid;
     c->st.passes = 1;
     if (refused(c, res.flags[FLBGPU_MAX_FILTERS])) return -1;
     if (settle(c, assume, res.flags, clean, &assume) >= 0) return 1;
-    if (l2m_merge(c)) return -1;
     if (res.total >= 0xfff00000ull) { set_err("result larger than 4 GiB%s%s", NULL, NULL); return -1; }
-    if (res.emitted && c->rtag_index >= 0 && ((c->active >> c->rtag_index) & 1)) {
-        fill_args(c, &a, c->d_in, bytes, res.n_valid);
-        if (rtag_collect(c, &a, res.n_valid, (res.flags[c->rtag_index] & CHF_CAUSE) != 0)) return -1;
-    }
     if (!res.emitted) {                              /* the result outgrew the output buffer: remember, let the general path do this call */
         c->small_cap_out = (size_t) res.total + (size_t) res.total / 4 + 4096;
         return 1;
     }
+    if (call_commit(c, &a, c->d_in, bytes, res.n_valid, res.flags)) return -1;
     c->st.records_out = res.n_out;
     c->st.bytes_out = res.total;
     *out_size = (size_t) res.total;
@@ -2543,19 +2558,25 @@ static int chain_do_one_by_one(flbgpu_chain *c, const void *data, size_t bytes, 
     *out_buf = owned; *out_size = cur_n;
     return FLBGPU_FILTER_MODIFIED;
 }
-#define FUSED_REFUSED_A_HANDED_OVER_VALUE(c) ((c)->nf > 1 && (c)->st.error_bits && !((c)->st.error_bits & ~(FLBGPU_E_FIELDS | FLBGPU_E_DEEP)))
+/* A fused call failed.  When all it refused were values an earlier filter of the chain made (FLBGPU_E_FIELDS, FLBGPU_E_DEEP),
+ * the filter-by-filter form redoes the call from an empty result; any other failure stands. */
+static int one_by_one_if_refused(flbgpu_chain *c, const void *data, size_t bytes, const char *tag, int tag_len, void **out_buf, size_t *out_size)
+{
+    if (!(c->nf > 1 && c->st.error_bits && !(c->st.error_bits & ~(FLBGPU_E_FIELDS | FLBGPU_E_DEEP)))) return -1;
+    *out_buf = NULL; *out_size = 0;
+    return chain_do_one_by_one(c, data, bytes, tag, tag_len, out_buf, out_size);
+}
 
 static int chain_do_locked(flbgpu_chain *c, const void *data, size_t bytes, const char *tag, int tag_len, void **out_buf, size_t *out_size)
 {
+    const char *sv;
+    int r;
     if (c->rtag_index == -2) return chain_do_one_by_one(c, data, bytes, tag, tag_len, out_buf, out_size);     /* one re-tagged stream per chain */
     if (c->ml_index >= 0) {
         /* a multiline filter makes new records out of runs of records: it runs on its own, the filters around it on what it made */
-        int r;
         if (c->ml_post) {
             r = ml_then_rest(c, data, NULL, bytes, NULL, 0, out_buf, out_size);
-            /* (a record the fused rest refuses -- a value an earlier filter of it made -- takes the filter-by-filter form) */
-            if (r < 0 && c->st.error_bits && !(c->st.error_bits & ~(FLBGPU_E_FIELDS | FLBGPU_E_DEEP))) { *out_buf = NULL; *out_size = 0; return chain_do_one_by_one(c, data, bytes, tag, tag_len, out_buf, out_size); }
-            return r;
+            return r < 0 ? one_by_one_if_refused(c, data, bytes, tag, tag_len, out_buf, out_size) : r;
         }
         if (c->nf > 1) return chain_do_one_by_one(c, data, bytes, tag, tag_len, out_buf, out_size);
         r = ml_run(c, data, NULL, bytes, NULL, 0, out_buf, out_size);
@@ -2566,34 +2587,18 @@ static int chain_do_locked(flbgpu_chain *c, const void *data, size_t bytes, cons
         c->tag_len = (uint32_t) (tag && tag_len > 0 ? tag_len : 0);
         if (bk_tag_upload(c->q, tag, c->tag_len, &c->d_tag)) { set_err("%s%s", bk_last_error(), NULL); return -1; }
     }
-    if (bytes <= small_bytes()) {
-        int ret = 0, r = chain_run_small(c, data, bytes, out_buf, out_size, &ret);
+    sv = getenv("FLBGPU_STREAM");
+    if (!(sv && sv[0] == '0')) {                     /* FLBGPU_STREAM=0: the two-pass form only */
+        int ret = 0;
+        r = bytes <= small_bytes() ? chain_run_small(c, data, bytes, out_buf, out_size, &ret) : chain_run_stream(c, data, bytes, out_buf, out_size, &ret);
+        bk_upload_end(c->q);                         /* `data` is not read after this call returns */
         if (r == 0) return ret;
-        if (r < 0) {
-            if (FUSED_REFUSED_A_HANDED_OVER_VALUE(c)) { *out_buf = NULL; *out_size = 0; return chain_do_one_by_one(c, data, bytes, tag, tag_len, out_buf, out_size); }
-            return -1;
-        }
-        *out_buf = NULL; *out_size = 0;
+        if (r < 0) return one_by_one_if_refused(c, data, bytes, tag, tag_len, out_buf, out_size);
+        *out_buf = NULL; *out_size = 0;              /* not for this form, or its speculation did not hold: the two-pass form */
     }
-    {
-        const char *sv = getenv("FLBGPU_STREAM");
-        if (!(sv && sv[0] == '0') && bytes > small_bytes()) {
-            int ret = 0, r = chain_run_stream(c, data, bytes, out_buf, out_size, &ret);
-            bk_upload_end(c->q);                     /* `data` is not read after this call returns */
-            if (r == 0) return ret;
-            if (r < 0) {
-                if (FUSED_REFUSED_A_HANDED_OVER_VALUE(c)) return chain_do_one_by_one(c, data, bytes, tag, tag_len, out_buf, out_size);
-                return -1;
-            }
-            *out_buf = NULL; *out_size = 0;          /* speculation did not hold: classic path */
-        }
-    }
-    {
-        int r = chain_run(c, data, NULL, bytes, NULL, 0, out_buf, out_size);
-        bk_upload_end(c->q);
-        if (r < 0 && FUSED_REFUSED_A_HANDED_OVER_VALUE(c)) { *out_buf = NULL; *out_size = 0; return chain_do_one_by_one(c, data, bytes, tag, tag_len, out_buf, out_size); }
-        return r;
-    }
+    r = chain_run(c, data, NULL, bytes, NULL, 0, out_buf, out_size);
+    bk_upload_end(c->q);
+    return r < 0 ? one_by_one_if_refused(c, data, bytes, tag, tag_len, out_buf, out_size) : r;
 }
 
 int flbgpu_chain_do(flbgpu_chain *c, const void *data, size_t bytes, const char *tag, int tag_len,

@@ -268,18 +268,9 @@ static int ml_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_ext,
     uint64_t total;
     struct timespec now;
 
-    memset(&c->st, 0, sizeof(c->st));
-    c->st.bytes_in = bytes;
-    *out_size = 0;
-    if (bytes >= 0xfff00000ull) { set_err("chunk larger than 4 GiB: split the append%s%s", NULL, NULL); return -1; }
-    if (d_in_ext) { d_in = d_in_ext; bk_upload_none(c->q); }
-    else {
-        if (dev_grow(c, (void **) &c->d_in, &c->cap_in, bytes + 64, 1, 0)) return -1;
-        d_in = c->d_in;
-        if (bk_upload_start(c->q, c->d_in, h_in, bytes)) return -1;
-    }
+    if (call_start(c, bytes, out_size, NULL) || !(d_in = place_input(c, h_in, d_in_ext, bytes))) return -1;
     if (bk_flags_clear(c->q, c->d_flags) || index_chunk(c, d_in, bytes, &n_rec, &off)) return -1;
-    REFUSE_WIDE_ARRAYS(h_in, d_in, return -1);
+    if (refuse_wide_arrays(c, h_in, d_in, off, bytes)) return -1;
     c->st.records_in = n_rec;
     c->st.passes = 1;
     if (n_rec == 0) return FLBGPU_FILTER_NOTOUCH;

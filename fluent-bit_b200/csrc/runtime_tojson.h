@@ -30,9 +30,7 @@ static int tj_run(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, int json_f
     char *res;
     int pass;
 
-    memset(&c->st, 0, sizeof(c->st));
-    c->st.bytes_in = bytes;
-    if (bytes >= 0xfff00000ull) { set_err("chunk larger than 4 GiB: split the append%s%s", NULL, NULL); return -1; }
+    if (call_start(c, bytes, out_size, NULL)) return -1;
     memset(&e, 0, sizeof(e));
     e.key_len = 0xffffffffu;
     if (date_key) {
@@ -48,7 +46,7 @@ static int tj_run(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, int json_f
     }
     d_in = c->d_in;
     if (bk_flags_clear(c->q, c->d_flags) || index_chunk(c, d_in, bytes, &n_rec, &off)) return -1;
-    REFUSE_WIDE_ARRAYS(h_in, d_in, return -1);
+    if (refuse_wide_arrays(c, h_in, d_in, off, bytes)) return -1;
     c->st.records_in = n_rec;
     total = 0;
     if (n_rec) {

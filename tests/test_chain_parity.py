@@ -13,6 +13,18 @@ import util
 pkg = util.pkg
 
 
+def per_filter(fs, chunk):
+    """the reference's own loop: one cb_filter per plugin, host buffers in between"""
+    cur, modified = chunk, False
+    for f in fs:
+        r, out = f.cb(cur)
+        if r == pkg.FILTER_MODIFIED:
+            cur, modified = out, True
+            if len(out) == 0:
+                break
+    return (pkg.FILTER_MODIFIED, cur) if modified else (pkg.FILTER_NOTOUCH, None)
+
+
 def run_case(lib, parsers, filters, chunk, fused=True):
     ctx = pkg.Context(0, lib=lib)
     ref = util.Ref()
@@ -23,18 +35,7 @@ def run_case(lib, parsers, filters, chunk, fused=True):
     for p, props in filters:
         ref.filter(p, props)
     want = ref.chain_do(chunk)
-    if fused:
-        got = ctx.chain(fs).do(chunk)
-    else:
-        # the reference's own loop: one cb_filter per plugin, host buffers in between
-        cur, modified = chunk, False
-        for f in fs:
-            r, out = f.cb(cur)
-            if r == pkg.FILTER_MODIFIED:
-                cur, modified = out, True
-                if len(out) == 0:
-                    break
-        got = (pkg.FILTER_MODIFIED, cur) if modified else (pkg.FILTER_NOTOUCH, None)
+    got = ctx.chain(fs).do(chunk) if fused else per_filter(fs, chunk)
     assert got[0] == want[0]
     assert got[1] == want[1]
 
@@ -241,6 +242,38 @@ def test_streaming_speculation_hostsim(sim_lib, ref_available, monkeypatch):
 @pytest.mark.gpu
 def test_streaming_speculation_gpu(gpu_lib, ref_available, monkeypatch):
     _speculation(gpu_lib, monkeypatch)
+
+
+def _fused_refusal_forms(lib, monkeypatch):
+    """A parser whose input an earlier filter of the chain made: the fused chain refuses, and each of its three forms
+    (small, streaming, two-pass) hands the call to the filter-by-filter form.  Two calls per chain object; the result is the
+    per-filter callbacks' every time."""
+    for name in ("docker_then_inner_json", "set_then_parse"):
+        _, parsers, filters, mk = [c for c in cases.CASES if c[0] == name][0]
+        block = mk()
+        chunk = block * ((3 << 20) // len(block) + 1)
+        ctx = pkg.Context(0, lib=lib)
+        for kw in parsers:
+            ctx.parser(**kw)
+        want = per_filter([ctx.filter(p, props) for p, props in filters], chunk)
+        for env in ({}, {"FLBGPU_SMALL_MB": "0", "FLBGPU_SLICE_MB": "1"}, {"FLBGPU_STREAM": "0"}):     # small, streaming, two-pass
+            for k in ("FLBGPU_SMALL_MB", "FLBGPU_SLICE_MB", "FLBGPU_STREAM"):
+                monkeypatch.delenv(k, raising=False)
+            for k, v in env.items():
+                monkeypatch.setenv(k, v)
+            chain = ctx.chain([ctx.filter(p, props) for p, props in filters])
+            for _ in range(2):
+                assert chain.do(chunk) == want, (name, env)
+                assert chain.stats().error_bits == 1, (name, env)       # FLBGPU_E_FIELDS: what the fused form refused
+
+
+def test_fused_refusal_forms_hostsim(sim_lib, monkeypatch):
+    _fused_refusal_forms(sim_lib, monkeypatch)
+
+
+@pytest.mark.gpu
+def test_fused_refusal_forms_gpu(gpu_lib, monkeypatch):
+    _fused_refusal_forms(gpu_lib, monkeypatch)
 
 
 def _json_sliced(lib, monkeypatch):

@@ -73,6 +73,40 @@ def test_l2m_golden_gpu(gpu_lib):
     check_golden(gpu_lib)
 
 
+def _forms_count_once(lib, monkeypatch, mode):
+    """log_to_metrics behind a filter that grows every record: the small form's result outgrows its output buffer and the
+    call moves to the two-pass form.  Each form (small, streaming, two-pass) counts every event of a call once."""
+    n = 200
+    props = l2m_cases.BASE + [("metric_mode", mode), ("label_field", "c")] + ([("value_field", "v")] if mode == "histogram" else [])
+    chunk = b"".join(util.event(1700000000 + i, 0, [(b"c", util.mp_str(b"red")), (b"v", b"\x01")]) for i in range(n))
+    texts = []
+    for env in ({}, {"FLBGPU_SMALL_MB": "0", "FLBGPU_SLICE_MB": "1"}, {"FLBGPU_STREAM": "0"}):     # small, streaming, two-pass
+        for k in ("FLBGPU_SMALL_MB", "FLBGPU_SLICE_MB", "FLBGPU_STREAM"):
+            monkeypatch.delenv(k, raising=False)
+        for k, v in env.items():
+            monkeypatch.setenv(k, v)
+        ctx = pkg.Context(0, lib=lib)
+        fs = [ctx.filter("modify", [("Add", "pad " + "p" * 400)]), ctx.filter("log_to_metrics", props)]
+        chain = ctx.chain(fs)
+        for call in (1, 2):
+            r, out = chain.do(chunk)
+            assert r == pkg.FILTER_MODIFIED and len(out) > len(chunk) + 400 * n
+            assert [s[2] for s in fs[1].l2m_sets()] == [n * call], (env, call)
+        texts.append(fs[1].l2m_text())
+    assert texts[1] == texts[0] and texts[2] == texts[0]
+
+
+@pytest.mark.parametrize("mode", ["counter", "histogram"])
+def test_l2m_forms_count_once_hostsim(mode, sim_lib, monkeypatch):
+    _forms_count_once(sim_lib, monkeypatch, mode)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mode", ["counter", "histogram"])
+def test_l2m_forms_count_once_gpu(mode, gpu_lib, monkeypatch):
+    _forms_count_once(gpu_lib, monkeypatch, mode)
+
+
 @pytest.mark.parametrize("bad", [
     [("metric_mode", "counter"), ("metric_description", "d")],                              # no tag
     [("metric_mode", "counter"), ("tag", "t")],                                             # no description
