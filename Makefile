@@ -28,10 +28,10 @@ $(PKG)/libflbgpu.so: $(CSRC)/kernels.o $(CSRC)/kernels_ml.o $(CSRC)/kernels_tojs
 	$(NVCC) $(ARCH) -shared -o $@ $(CSRC)/kernels.o $(CSRC)/kernels_ml.o $(CSRC)/kernels_tojson.o $(CSRC)/kernels_lines.o $(CSRC)/runtime.o $(CSRC)/rx_compile.o -lcudart -lpthread -ldl
 
 hostsim: tests/hostsim/libhostsim.so
-tests/hostsim/libhostsim.so: tests/hostsim/hostsim.cpp tests/hostsim/hostsim_tail.cpp $(CSRC)/runtime.c $(CSRC)/rx_compile.c $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h)
+tests/hostsim/libhostsim.so: tests/hostsim/hostsim.cpp tests/hostsim/hostsim_tail.cpp tests/hostsim/hostsim_gelf.cpp $(CSRC)/runtime.c $(CSRC)/rx_compile.c $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h)
 	gcc $(CFLAGS) -c $(CSRC)/runtime.c -o tests/hostsim/runtime.o
 	gcc $(CFLAGS) -c $(CSRC)/rx_compile.c -o tests/hostsim/rx_compile.o
-	g++ $(CFLAGS) -shared -o $@ tests/hostsim/hostsim.cpp tests/hostsim/hostsim_tail.cpp tests/hostsim/runtime.o tests/hostsim/rx_compile.o -lrt -lpthread
+	g++ $(CFLAGS) -shared -o $@ tests/hostsim/hostsim.cpp tests/hostsim/hostsim_tail.cpp tests/hostsim/hostsim_gelf.cpp tests/hostsim/runtime.o tests/hostsim/rx_compile.o -lrt -lpthread
 
 # the same emulation under AddressSanitizer + UBSan (host runtime and the device code as the CPU compiles it):
 #   make hostsim-asan && FLBGPU_HOSTSIM_SO=/tmp/flbgpu-asan/libhostsim.so LD_PRELOAD=$$(gcc -print-file-name=libasan.so) \
@@ -41,7 +41,7 @@ hostsim-asan:
 	mkdir -p /tmp/flbgpu-asan
 	gcc $(SAN) -c $(CSRC)/runtime.c -o /tmp/flbgpu-asan/runtime.o
 	gcc $(SAN) -c $(CSRC)/rx_compile.c -o /tmp/flbgpu-asan/rx_compile.o
-	g++ $(SAN) -shared -o /tmp/flbgpu-asan/libhostsim.so tests/hostsim/hostsim.cpp tests/hostsim/hostsim_tail.cpp /tmp/flbgpu-asan/runtime.o /tmp/flbgpu-asan/rx_compile.o
+	g++ $(SAN) -shared -o /tmp/flbgpu-asan/libhostsim.so tests/hostsim/hostsim.cpp tests/hostsim/hostsim_tail.cpp tests/hostsim/hostsim_gelf.cpp /tmp/flbgpu-asan/runtime.o /tmp/flbgpu-asan/rx_compile.o
 
 # the emulation with "device" allocations filled with a byte pattern (cudaMalloc does not hand out zeroes; a fresh malloc often does):
 #   make hostsim-poison && FLBGPU_HOSTSIM_SO=/tmp/flbgpu-poison/libhostsim.so python -m pytest tests -q -m "not gpu"
@@ -49,11 +49,11 @@ hostsim-poison:
 	mkdir -p /tmp/flbgpu-poison
 	gcc $(CFLAGS) -c $(CSRC)/runtime.c -o /tmp/flbgpu-poison/runtime.o
 	gcc $(CFLAGS) -c $(CSRC)/rx_compile.c -o /tmp/flbgpu-poison/rx_compile.o
-	g++ $(CFLAGS) -DHS_POISON=0xA5 -shared -o /tmp/flbgpu-poison/libhostsim.so tests/hostsim/hostsim.cpp tests/hostsim/hostsim_tail.cpp /tmp/flbgpu-poison/runtime.o /tmp/flbgpu-poison/rx_compile.o -lrt -lpthread
+	g++ $(CFLAGS) -DHS_POISON=0xA5 -shared -o /tmp/flbgpu-poison/libhostsim.so tests/hostsim/hostsim.cpp tests/hostsim/hostsim_tail.cpp tests/hostsim/hostsim_gelf.cpp /tmp/flbgpu-poison/runtime.o /tmp/flbgpu-poison/rx_compile.o -lrt -lpthread
 
 ORC_SRC = oracle/flb_oracle.c oracle/orc_parsers.c oracle/orc_regex.c oracle/orc_time.c oracle/orc_msgpack.c
 oracle: oracle/liboracle.so
-	@if [ -d /root/reference ]; then $(MAKE) -s -C oracle/refshim && $(MAKE) -s -C oracle/refshim -f tail.mk tail; else echo "oracle/_ref: reference tree absent, using prebuilt"; fi
+	@if [ -d /root/reference ]; then $(MAKE) -s -C oracle/refshim && $(MAKE) -s -C oracle/refshim -f tail.mk tail && $(MAKE) -s -C oracle/refshim -f gelf.mk gelf; else echo "oracle/_ref: reference tree absent, using prebuilt"; fi
 oracle/liboracle.so: $(ORC_SRC) oracle/orc.h oracle/orc_flb.h
 	gcc $(CFLAGS) -shared -o $@ $(ORC_SRC) -lm
 

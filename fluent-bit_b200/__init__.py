@@ -43,6 +43,12 @@ class Stats(C.Structure):
                 ("error_bits", C.c_uint32), ("phase_ms", C.c_float * 4)]
 
 
+class GelfFields(C.Structure):
+    """struct flbgpu_gelf_fields (struct flb_gelf_fields): None = the default name"""
+    _fields_ = [("timestamp_key", C.c_char_p), ("host_key", C.c_char_p), ("short_message_key", C.c_char_p),
+                ("full_message_key", C.c_char_p), ("level_key", C.c_char_p)]
+
+
 EXPORTS = [
     "flbgpu_init", "flbgpu_shutdown", "flbgpu_last_error", "flbgpu_backend_name", "flbgpu_device_count",
     "flbgpu_parser_create", "flbgpu_parser_get", "flbgpu_parser_do", "flbgpu_parser_do_batch", "flbgpu_parser_destroy",
@@ -54,7 +60,7 @@ EXPORTS = [
     "flbgpu_comm_unique_id", "flbgpu_comm_init", "flbgpu_l2m_allreduce",
     "flbgpu_pack_state_init", "flbgpu_pack_state_reset", "flbgpu_pack_json_state", "flbgpu_pack_json_state_batch",
     "flbgpu_ml_parser_create", "flbgpu_ml_parser_rule", "flbgpu_ml_parser_init", "flbgpu_ml_set_buffer_limit",
-    "flbgpu_msgpack_to_json_format", "flbgpu_lines_to_events", "flbgpu_lines_to_events_parsed", "flbgpu_chain_set_result_buffer",
+    "flbgpu_msgpack_to_json_format", "flbgpu_msgpack_to_gelf", "flbgpu_lines_to_events", "flbgpu_lines_to_events_parsed", "flbgpu_chain_set_result_buffer",
     "flbgpu_pool_new", "flbgpu_pool_do", "flbgpu_pool_destroy",
 ]
 
@@ -110,6 +116,8 @@ def load(path=None):
     L.flbgpu_ml_parser_init.argtypes = [vp]
     L.flbgpu_ml_set_buffer_limit.argtypes = [vp, sz]
     L.flbgpu_msgpack_to_json_format.argtypes = [vp, vp, sz, C.c_int, C.c_int, cp, C.c_int, C.POINTER(vp), C.POINTER(sz), C.POINTER(sz)]
+    L.flbgpu_msgpack_to_gelf.argtypes = [vp, vp, sz, C.POINTER(GelfFields), cp, cp, sz, C.c_int, C.POINTER(vp), C.POINTER(sz),
+                                         C.POINTER(sz), C.POINTER(sz)]
     L.flbgpu_lines_to_events.argtypes = [vp, vp, sz, cp, C.c_int, C.c_int64, C.c_int64, cp, cp, cp, C.c_uint64, C.POINTER(vp), C.POINTER(sz),
                                          C.POINTER(sz), C.POINTER(sz)]
     L.flbgpu_lines_to_events_parsed.argtypes = [vp, vp, sz, cp, C.c_int, C.c_int64, C.c_int64, cp, cp, cp, C.c_uint64, C.POINTER(vp),
@@ -246,6 +254,26 @@ class Context:
         text = C.string_at(out.value, n.value)
         _libc.free(out)
         return text, und.value
+
+    def to_gelf(self, data, fields=None, tag_key=None, tag=None, separator=b"\n"):
+        """flb_msgpack_to_gelf() on every event, as out_gelf / out_http flush a chunk: (text bytes or None, events that failed,
+        events with a string whose text is undefined in the reference).  fields: dict of GelfFields' names (missing or None =
+        the default name); separator: b"\n" (out_http) or b"\0" (out_gelf over TCP / TLS)."""
+        out, n, failed, und = C.c_void_p(), C.c_size_t(), C.c_size_t(), C.c_size_t()
+        buf = C.create_string_buffer(data, len(data))
+        f = GelfFields(**{k: _b(v) for k, v in (fields or {}).items()}) if fields is not None else None
+        tag = _b(tag)
+        sep = separator[0] if isinstance(separator, (bytes, bytearray)) else int(separator)
+        r = self.L.flbgpu_msgpack_to_gelf(self.h, C.cast(buf, C.c_void_p), len(data), C.byref(f) if f is not None else None, _b(tag_key),
+                                          tag, len(tag) if tag is not None else 0, sep, C.byref(out), C.byref(n), C.byref(failed),
+                                          C.byref(und))
+        if r < 0:
+            raise FlbGpuError("msgpack_to_gelf: %s" % self.err())
+        if r == 1:
+            return None, failed.value, und.value
+        text = C.string_at(out.value, n.value)
+        _libc.free(out)
+        return text, failed.value, und.value
 
     def ml_parser(self, name, type="regex", rules=(), match_string=None, negate=False, flush_ms=0, key_content=None,
                   key_group=None, key_pattern=None, parser=None):

@@ -313,25 +313,34 @@ FLB_HD uint32_t tj_datetime(int64_t sec, uint64_t usec, int iso, uint8_t *o)
 }
 
 
+/* the timestamp at q of an event rec_frame() accepted, as flb_log_event_decoder_decode_timestamp() converts it; returns the
+ * position behind it */
+FLB_HD const uint8_t *tj_event_time(const uint8_t *q, const uint8_t *end, int64_t *sec, int64_t *nsec)
+{
+    struct mp_tok t;
+    mp_token(q, end, &t);
+    *nsec = 0;
+    if (t.type == MPT_UINT || t.type == MPT_INT) *sec = (int64_t) t.u;
+    else if (t.type == MPT_F64) {
+        union { uint64_t u; double d; } cv;
+        cv.u = t.u;
+        *sec = mp_d2i64(cv.d);
+        *nsec = mp_d2i64((cv.d - (double) *sec) * 1000000000.0);
+    }
+    else { *sec = (int64_t) (int32_t) mp_be32(q + t.hdr); *nsec = (int64_t) (int32_t) mp_be32(q + t.hdr + 4); }
+    return q + t.hdr + (t.type == MPT_EXT ? t.len : 0);
+}
+
 /* the event as one msgpack map in its scratch slice (flb_pack.c:1380-1497); returns its length */
 FLB_HDN uint32_t tj_pack_event(const struct tj_env *e, uint32_t i, uint8_t *b)
 {
     const uint8_t *p = e->in + e->off[i], *end = p + e->len[i], *q = p + 1, *meta = 0, *meta_end = 0;
     struct mp_tok t;
-    int64_t sec, nsec = 0;
+    int64_t sec, nsec;
     uint32_t n = 5, entries = 0, k;
     const int v2 = (*q == 0x92);
     if (v2) q++;
-    mp_token(q, end, &t);
-    if (t.type == MPT_UINT || t.type == MPT_INT) sec = (int64_t) t.u;
-    else if (t.type == MPT_F64) {
-        union { uint64_t u; double d; } cv;
-        cv.u = t.u;
-        sec = mp_d2i64(cv.d);
-        nsec = mp_d2i64((cv.d - (double) sec) * 1000000000.0);
-    }
-    else { sec = (int64_t) (int32_t) mp_be32(q + t.hdr); nsec = (int64_t) (int32_t) mp_be32(q + t.hdr + 4); }
-    q += t.hdr + (t.type == MPT_EXT ? t.len : 0);
+    q = tj_event_time(q, end, &sec, &nsec);
     if (v2) { meta = q; q = mp_skip(q, end); meta_end = q; }
     if (e->key_len != 0xffffffffu) {
         n += mp_put_str_hdr(b + n, e->key_len);

@@ -208,6 +208,11 @@ int bk_ml_emit(bk_q *q, const struct ml_env *e, uint32_t n_ev, const uint64_t *d
  * slice, e->size[i] = bytes of its text; emit: event i at d_out + d_bsum[i / BK_REC_BLOCK] + (sizes before it in its block). */
 int bk_tj_sizes(bk_q *q, const struct tj_env *e);
 int bk_tj_emit(bk_q *q, const struct tj_env *e, const uint64_t *d_bsum, uint8_t *d_out);
+/* chunk -> GELF messages (dev_gelf.cuh), asynchronous on the queue's stream.  sizes: e->size[i] = bytes of event i's message
+ * and separator, 0 for an event left out (counted in e->failed when the reference returns NULL for it); emit: event i at
+ * d_out + d_bsum[i / BK_REC_BLOCK] + (sizes before it in its block). */
+int bk_gf_sizes(bk_q *q, const struct gf_env *e);
+int bk_gf_emit(bk_q *q, const struct gf_env *e, const uint64_t *d_bsum, uint8_t *d_out);
 
 /* raw text -> log events (dev_lines.cuh), asynchronous on the queue's stream.  count: e->cnt[t] per tile; fill: e->nl[] from the
  * tile offsets (d_bsum per BK_REC_BLOCK tiles); sizes: e->size[k] per line; emit: line k's event at d_out + d_bsum[k / BK_REC_BLOCK]

@@ -379,6 +379,37 @@ struct tj_env {
 #define TJ_DATE_EPOCH_MS 4u
 #define TJ_SCR_PAD(key_len) ((key_len) + 128u)
 
+/* ---------------------------------------------------- chunk -> GELF messages (dev_gelf.cuh) */
+#define GF_KEY_MAX 128u               /* bytes of a field key or of the tag key */
+#define GF_TAG_MAX 256u               /* bytes of the tag */
+#define GF_NONE 0xffffffffu
+/* the five field keys in the order flb_msgpack_to_gelf() tests them (src/flb_pack_gelf.c:522-606) */
+#define GF_HOST 0
+#define GF_SHORT 1
+#define GF_TIMESTAMP 2
+#define GF_LEVEL 3
+#define GF_FULL 4
+struct gf_env {
+    const uint8_t *in;
+    uint64_t in_len;                  /* the chunk's end: what the string writer may read up to without tag_key */
+    const uint32_t *off, *len; const uint8_t *kind;
+    uint32_t n_rec;
+    uint8_t *scr;                     /* tag_key: event i re-packed with the tag at scr + off[i] + i * scr_pad */
+    uint32_t scr_pad;
+    uint32_t *plen;                   /* bytes of that map */
+    uint32_t *size;                   /* bytes of text per event (separator included), 0: left out */
+    uint32_t *err;
+    unsigned long long *undefined;    /* events with a string whose text depends, in the reference, on memory behind its buffer */
+    unsigned long long *failed;       /* events flb_msgpack_to_gelf() returns NULL for */
+    uint32_t sep;                     /* the byte behind each message */
+    uint32_t fkey_len[5];             /* GF_HOST ...: the names the record's keys are matched against */
+    uint8_t fkey[5][GF_KEY_MAX];
+    uint32_t tag_key_len;             /* GF_NONE: no tag_key */
+    uint8_t tag_key[GF_KEY_MAX];
+    uint32_t tag_len;
+    uint8_t tag[GF_TAG_MAX];
+};
+
 /* ---------------------------------------------------- raw text -> log events (dev_lines.cuh) */
 #define LN_TILE 256u
 struct ln_env {

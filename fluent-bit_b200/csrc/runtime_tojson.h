@@ -144,3 +144,117 @@ int flbgpu_msgpack_to_json_format(flbgpu_ctx *ctx, const void *data, size_t byte
     pthread_mutex_unlock(&c->lock);
     return r;
 }
+
+/* ---- chunk -> GELF messages: flb_msgpack_to_gelf() (src/flb_pack_gelf.c) on every event, as out_gelf and out_http flush a
+ * chunk ---- */
+
+static int gf_copy_key(uint8_t *dst, uint32_t *len, const char *key, const char *what)
+{
+    const size_t kl = strlen(key);
+    if (kl > GF_KEY_MAX) { set_err("%s longer than 128 bytes%s", what, NULL); return -1; }
+    memcpy(dst, key, kl);
+    *len = (uint32_t) kl;
+    return 0;
+}
+
+/* the call's arguments as the kernels take them (e->in and the buffers are set by gelf_run) */
+static int gf_args(struct gf_env *e, const struct flbgpu_gelf_fields *fields, const char *tag_key, const char *tag, size_t tag_len,
+                   int separator)
+{
+    static const char *const names[5] = { "host", "short_message", "timestamp", "level", "full_message" };   /* GF_HOST ... */
+    const char *keys[5] = { NULL, NULL, NULL, NULL, NULL };
+    int k;
+    memset(e, 0, sizeof(*e));
+    if (separator != 0 && separator != '\n') { set_err("separator must be 0 (out_gelf over TCP / TLS) or '\\n' (out_http)%s%s", NULL, NULL); return -1; }
+    e->sep = (uint32_t) separator;
+    if (fields) {
+        keys[GF_HOST] = fields->host_key; keys[GF_SHORT] = fields->short_message_key; keys[GF_TIMESTAMP] = fields->timestamp_key;
+        keys[GF_LEVEL] = fields->level_key; keys[GF_FULL] = fields->full_message_key;
+    }
+    for (k = 0; k < 5; k++)
+        if (gf_copy_key(e->fkey[k], &e->fkey_len[k], keys[k] ? keys[k] : names[k], "a GELF field key")) return -1;
+    e->tag_key_len = GF_NONE;
+    if (tag_key) {
+        if (!tag) { set_err("tag_key is set but the tag is NULL%s%s", NULL, NULL); return -1; }
+        if (gf_copy_key(e->tag_key, &e->tag_key_len, tag_key, "tag_key")) return -1;
+        if (tag_len > GF_TAG_MAX) { set_err("tag longer than 256 bytes%s%s", NULL, NULL); return -1; }
+        memcpy(e->tag, tag, tag_len);
+        e->tag_len = (uint32_t) tag_len;
+    }
+    return 0;
+}
+
+static int gelf_run(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, struct gf_env *e, char **out, size_t *out_size,
+                    size_t *failed, size_t *undefined_strings)
+{
+    const uint8_t *d_in = c->d_in;
+    uint32_t n_rec, h_flags[FLBGPU_MAX_FILTERS + 1];
+    size_t off;
+    unsigned long long cnt[2] = { 0, 0 };
+    uint64_t total = 0;
+    char *res;
+
+    if (call_start(c, bytes, out_size, NULL)) return -1;
+    if (bytes && !(d_in = place_input(c, h_in, NULL, bytes))) return -1;
+    if (bk_flags_clear(c->q, c->d_flags) || index_chunk(c, d_in, bytes, &n_rec, &off)) return -1;
+    if (refuse_wide_arrays(c, h_in, d_in, off, bytes)) return -1;
+    c->st.records_in = n_rec;
+    if (n_rec) {
+        e->in = d_in; e->in_len = bytes; e->off = c->d_off; e->len = c->d_len; e->kind = c->d_kind; e->n_rec = n_rec;
+        e->err = c->d_flags + FLBGPU_MAX_FILTERS;
+        e->size = c->d_size;
+        /* work memory: the two counters (undefined strings, failed events), then the re-packed lengths */
+        if (dev_grow(c, (void **) &c->d_mlw, &c->cap_mlw, 16 + sizeof(uint32_t) * (size_t) n_rec + 64, 1, 0)) return -1;
+        e->undefined = (unsigned long long *) c->d_mlw; e->failed = e->undefined + 1;
+        e->plen = (uint32_t *) (c->d_mlw + 16);
+        if (e->tag_key_len != GF_NONE) {
+            /* a re-packed event is its body (canonical encodings are never longer), a map header up to 4 bytes longer and
+             * the two strings with their headers */
+            e->scr_pad = 4 + 5 + e->tag_key_len + 5 + e->tag_len + 64;
+            if (dev_grow(c, (void **) &c->d_scr, &c->cap_scr, bytes + (size_t) n_rec * e->scr_pad + 64, 1, 0)) return -1;
+            e->scr = c->d_scr;
+        }
+        if (bk_zero(c->q, e->undefined, 16) || bk_gf_sizes(c->q, e) || bk_flags_fetch(c->q, c->d_flags, h_flags)) return -1;
+        if (refused(c, h_flags[FLBGPU_MAX_FILTERS])) return -1;
+        if (sizes_to_offsets(c, c->d_size, n_rec, NULL, NULL, "result larger than 4 GiB", &total)) return -1;
+        if (bk_d2h(c->q, cnt, e->undefined, sizeof(cnt)) || bk_sync(c->q)) return -1;
+    }
+    bk_upload_end(c->q);
+    c->st.kernel_launches = bk_launch_count();
+    if (failed) *failed = (size_t) cnt[1];
+    if (undefined_strings) *undefined_strings = (size_t) cnt[0];
+    if (total == 0) return 1;
+    res = malloc((size_t) total + 1);
+    if (!res) { set_err("out of memory%s%s", NULL, NULL); return -1; }
+    if (dev_grow(c, (void **) &c->d_out, &c->cap_out, total, 1, 0) || bk_gf_emit(c->q, e, c->d_bsum, c->d_out) ||
+        bk_d2h(c->q, res, c->d_out, (size_t) total) || bk_sync(c->q)) { free(res); return -1; }
+    res[total] = 0;
+    *out = res; *out_size = (size_t) total;
+    c->st.bytes_out = total;
+    return 0;
+}
+
+/* 0: *out is the malloc()ed, NUL-terminated text; 1: no event was converted; -1: the call failed (flbgpu_last_error) */
+int flbgpu_msgpack_to_gelf(flbgpu_ctx *ctx, const void *data, size_t bytes, const struct flbgpu_gelf_fields *fields,
+                           const char *tag_key, const char *tag, size_t tag_len, int separator,
+                           char **out, size_t *out_size, size_t *failed, size_t *undefined_strings)
+{
+    struct gf_env e;
+    flbgpu_chain *c;
+    int r;
+    g_rt_err[0] = 0;
+    if (!ctx || !out || !out_size || (!data && bytes)) return -1;
+    *out = NULL; *out_size = 0;
+    if (failed) *failed = 0;
+    if (undefined_strings) *undefined_strings = 0;
+    if (gf_args(&e, fields, tag_key, tag, tag_len, separator)) return -1;
+    c = tj_chain(ctx);
+    if (!c) return -1;
+
+    pthread_mutex_lock(&c->lock);
+    ctx->last_q = c->q;
+    r = gelf_run(c, data, bytes, &e, out, out_size, failed, undefined_strings);
+    if (r < 0) bk_upload_end(c->q);
+    pthread_mutex_unlock(&c->lock);
+    return r;
+}

@@ -131,6 +131,28 @@ int  flbgpu_pack_json_state_batch(flbgpu_ctx *ctx, int n, const char *const *js,
 int flbgpu_msgpack_to_json_format(flbgpu_ctx *ctx, const void *data, size_t bytes, int json_format, int date_format,
                                   const char *date_key, int escape_unicode, char **out, size_t *out_size, size_t *undefined_strings);
 
+/* ---- output side: a chunk as GELF messages -------------------------------------------------------------------------
+ * flb_msgpack_to_gelf(), src/flb_pack_gelf.c, on every event the log event decoder yields, in order -- the flush loops of
+ * out_gelf (plugins/out_gelf/gelf.c:265-392) and out_http `format gelf` (plugins/out_http/http.c:378-440).  Each message is
+ * followed by one `separator` byte: '\n' for out_http, 0 for out_gelf over TCP / TLS (it writes the NUL behind each message).
+ * struct flbgpu_gelf_fields mirrors struct flb_gelf_fields (include/fluent-bit/flb_pack.h:119); a NULL member, or a NULL
+ * `fields`, is the default name.  tag_key (out_gelf's `tag_key`): the body is re-encoded with `tag_key: tag` behind its members
+ * first, as inject_tag() does.  Keys are at most 128 bytes, the tag at most 256.
+ * An event the reference returns NULL for (no short message, a level that is neither a non-negative integer nor a string, a
+ * top-level float longer than 48 characters as "%f") is left out and counted in *failed: out_gelf skips it, out_http fails the
+ * whole payload (its caller treats *failed > 0 as FLB_ERROR).  *undefined_strings as for flbgpu_msgpack_to_json_format().
+ * Returns 0 with *out = malloc()ed NUL-terminated text of *out_size bytes, 1 when no event was converted, -1 on failure. */
+struct flbgpu_gelf_fields {
+    const char *timestamp_key;
+    const char *host_key;
+    const char *short_message_key;
+    const char *full_message_key;
+    const char *level_key;
+};
+int flbgpu_msgpack_to_gelf(flbgpu_ctx *ctx, const void *data, size_t bytes, const struct flbgpu_gelf_fields *fields,
+                           const char *tag_key, const char *tag, size_t tag_len, int separator,
+                           char **out, size_t *out_size, size_t *failed, size_t *undefined_strings);
+
 /* ---- input side: raw text as log events -------------------------------------------------------------------------
  * The line loop of in_tail, plugins/in_tail/tail_file.c process_content() :629-700 and flb_tail_file_pack_line() :338-391, for
  * the plain case (no parser, no docker mode, none of the tail's own multiline modes): the text is cut at '\n'; with
