@@ -44,9 +44,9 @@ struct bk_chain_args {
     uint32_t active;              /* bit k: filter k sees this call's chunk (Match routing) */
     uint32_t defer_ok;            /* a record may be put off to the follow-up launch before the first JSON parser runs (nothing
                                      with side effects -- log_to_metrics -- comes earlier in the chain) */
-    uint32_t split;               /* evaluate as two launches: filter 0 (the parser), then the rest (the capture cache has
-                                     RC_CACHE_MAXF columns more than cap_stride) */
-    uint32_t split_list;          /* ... and the head launch holds grep filters too: the tail launch runs over the list of records it left */
+    uint32_t split;               /* evaluate as two launches: filter 0 (the parser) and the grep filters right behind it, then
+                                     the rest over the list of records the first left (the capture cache has RC_CACHE_MAXF
+                                     columns more than cap_stride) */
     const uint32_t *d_off;        /* record index */
     const uint32_t *d_len;
     const uint8_t *d_kind;

@@ -340,7 +340,7 @@ struct k_chain_params {
     uint32_t bm_words;           /* JSON stage 1: 32-bit words of string-event bitmap per warp in shared memory, 0 = none */
     uint32_t *defer_list;        /* records put off by the stage-2 walker (CH_DEFER), and how many */
     unsigned long long *defer_cnt;
-    uint32_t *tlist, *tn;        /* split evaluation with grep filters in the head launch: the records that are still there, for the tail launch */
+    uint32_t *tlist, *tn;        /* split evaluation: the records the head launch left for the tail launch, and how many */
     uint32_t n_rec;
     const uint32_t *n_dev;       /* small form: the record count lives on the device */
     uint32_t *size;
@@ -393,7 +393,9 @@ __global__ void __launch_bounds__(1024, 1) k_chain_eval_t(const __grid_constant_
     const uint32_t n_rec = p.n_dev ? *p.n_dev : p.n_rec;
     uint32_t i = p.r0 + blockIdx.x * blockDim.x + threadIdx.x;
     bool valid = i < n_rec;
-    if (PH == CH_PH_TAIL && p.tlist) {               /* dense: lane t takes the t-th record the head launch left */
+    if (PH == CH_PH_TAIL) {
+        /* dense: lane t takes the t-th record the head launch left.  The tail reads nothing of a record that is not on the
+         * list: the follow-up launch beside it writes the size and the cache row of the records the head put off. */
         const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
         valid = t < *p.tn;
         i = valid ? p.tlist[t] : 0;
@@ -435,9 +437,6 @@ __global__ void __launch_bounds__(1024, 1) k_chain_eval_t(const __grid_constant_
     if (!valid) return;
     uint32_t sz = 0;
     if (PH != CH_PH_TAIL && !live && p.env.esize) p.env.esize[i] = 0;      /* an event the decoder steps over has no entry of its own */
-    if (PH == CH_PH_TAIL) {
-        if (!live || p.size[i] == 0) return;           /* dropped by the head launch, or handed to the follow-up launch */
-    }
     if (live) {
         /* the environment is read where the kernel parameters live (__grid_constant__: no per-lane copy); what differs per
          * lane travels in a few words */
@@ -449,10 +448,10 @@ __global__ void __launch_bounds__(1024, 1) k_chain_eval_t(const __grid_constant_
         if (sz == CH_DEFER) {                          /* the follow-up launch evaluates it whole, with the byte scanner */
             p.defer_list[atomicAdd(p.defer_cnt, 1ull)] = i;
             if (PH != CH_PH_HEAD) return;
-            sz = 0;                                    /* the tail launch steps over it */
+            sz = 0;                                    /* kept off the tail launch's list */
         }
     }
-    if (PH == CH_PH_HEAD && p.tlist) {
+    if (PH == CH_PH_HEAD) {
         /* the survivors of the warp go to the tail launch's list side by side (one atomic per warp; the order of the warps in
          * the list does not matter: every record owns its slots) */
         const unsigned lanes = __activemask();
@@ -1420,7 +1419,7 @@ static int defer_setup(bk_q *q, k_chain_params *p, const struct bk_chain_args *a
     }
     CK(cudaMemsetAsync(q->dtotal + 9, 0, sizeof(unsigned long long) * 2, st));       /* [9] records put off, [10] records left for the tail launch */
     p->defer_list = q->d_defer; p->defer_cnt = q->dtotal + 9;
-    if (a->split && a->split_list) {
+    if (a->split) {
         if (q->cap_tlist < n) {
             CK(cudaStreamSynchronize(q->stream));
             cudaFree(q->d_tlist); q->d_tlist = 0; q->cap_tlist = 0;
@@ -1446,7 +1445,7 @@ int bk_chain_eval(bk_q *q, const struct bk_chain_args *a, uint32_t r0, uint32_t 
         const unsigned grid = (r1 - r0 + q->eval_block - 1) / q->eval_block;
         k_chain_eval_t<CH_PH_HEAD><<<grid, q->eval_block, (size_t) p.bm_words * 4 * (q->eval_block / 32), q->stream>>>(p);
         /* the records the head put off (a few per cent, one long lane each: ~200 us per slice with most of the GPU idle) are
-         * evaluated BESIDE the tail launch -- the two touch different records */
+         * evaluated BESIDE the tail launch -- the two touch different records: the tail only those on the head's list */
         CK(cudaEventRecord(q->d_ev[0], q->stream));
         CK(cudaStreamWaitEvent(q->dstream, q->d_ev[0], 0));
         k_chain_eval_deferred<<<q->n_sm * 4, BK_REC_BLOCK, 0, q->dstream>>>(p);

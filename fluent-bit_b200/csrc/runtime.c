@@ -176,7 +176,6 @@ struct flbgpu_chain {
     uint32_t cap_stride;
     int needs_scratch;
     uint32_t scr_mul;
-    int split_list;                           /* ... with grep filters in the first: the second runs over the list of survivors */
     int split;                                /* evaluation in two launches: the parser (filter 0), then the other filters */
     int defer_ok;                             /* no log_to_metrics filter in front of a parser filter: records may be re-evaluated from scratch */
     uint8_t *d_scr; size_t cap_scr;
@@ -1504,7 +1503,6 @@ int flbgpu_chain_init(flbgpu_chain *c)
              * is never handed over */
             h.split_at = 1;
             if (c->split) while ((int) h.split_at < c->nf && c->f[h.split_at]->kind == FLBGPU_F_GREP) h.split_at++;
-            c->split_list = c->split && h.split_at > 1;
         }
     }
     h.n_filters = c->nf;
@@ -1769,7 +1767,6 @@ static void fill_args(flbgpu_chain *c, struct bk_chain_args *a, const uint8_t *d
     a->scr_mul = c->scr_mul ? c->scr_mul : 4;
     a->defer_ok = (uint32_t) c->defer_ok;
     a->split = (uint32_t) c->split;
-    a->split_list = (uint32_t) c->split_list;
     a->d_esize = (c->rtag_index >= 0 && ((c->active >> c->rtag_index) & 1)) ? c->d_esize : NULL;
     a->d_tag = c->d_tag; a->tag_len = c->tag_len;
     a->d_prep = c->want_report ? c->d_prep : NULL;

@@ -229,22 +229,33 @@ int bk_chain_eval(bk_q *, const struct bk_chain_args *a, uint32_t r0, uint32_t r
     }
     if (a->d_esize) for (i = r0; i < r1; i++) if (a->d_kind[i] != 0) a->d_esize[i] = 0;
     if (a->split) {
-        /* the three launches of the split form, in the kernel's order: head over all records, tail, then the records the
-         * head put off, whole */
-        uint8_t *put_off = (uint8_t *) calloc(r1 - r0 + 1, 1);
+        /* the three launches of the split form: the head over all records, which lists the records it keeps for the tail
+         * and those it puts off; the tail over its list; the put-off records, whole.  The kernel runs the last two side by
+         * side on two streams, so either may finish first: FLBGPU_SIM_DEFER_FIRST=1 runs the put-off records before the tail. */
+        const int defer_first = getenv("FLBGPU_SIM_DEFER_FIRST") && getenv("FLBGPU_SIM_DEFER_FIRST")[0] == '1';
+        uint32_t *tlist = (uint32_t *) malloc(sizeof(uint32_t) * (r1 - r0 + 1)), *dlist = (uint32_t *) malloc(sizeof(uint32_t) * (r1 - r0 + 1));
+        uint32_t tn = 0, dn = 0, t;
         for (i = r0; i < r1; i++) {
             uint32_t sz = 0;
             if (a->d_kind[i] == 0) ln.raw_lo = hs_raw_lo(a, i), sz = chain_record<false, CH_PH_HEAD>(&e, &ln, i, a->d_off[i], a->d_len[i], 0);
-            if (sz == CH_DEFER) { put_off[i - r0] = 1; sz = 0; }
+            if (sz == CH_DEFER) { dlist[dn++] = i; sz = 0; }
+            if (sz) tlist[tn++] = i;
             a->d_size[i] = sz;
         }
-        for (i = r0; i < r1; i++)
-            if (a->d_kind[i] == 0 && a->d_size[i]) a->d_size[i] = chain_record<false, CH_PH_TAIL>(&e, &ln, i, a->d_off[i], a->d_len[i], 0);
-        for (i = r0; i < r1; i++)
-            if (put_off[i - r0]) { struct ch_lane plain; memset(&plain, 0, sizeof(plain)); plain.raw_lo = hs_raw_lo(a, i); a->d_size[i] = chain_record<false>(&e, &plain, i, a->d_off[i], a->d_len[i], 0); }
+        for (int pass = 0; pass < 2; pass++) {
+            if (pass == (defer_first ? 1 : 0))
+                for (t = 0; t < tn; t++) i = tlist[t], a->d_size[i] = chain_record<false, CH_PH_TAIL>(&e, &ln, i, a->d_off[i], a->d_len[i], 0);
+            else for (t = 0; t < dn; t++) {
+                struct ch_lane plain;
+                memset(&plain, 0, sizeof(plain));
+                i = dlist[t];
+                plain.raw_lo = hs_raw_lo(a, i);
+                a->d_size[i] = chain_record<false>(&e, &plain, i, a->d_off[i], a->d_len[i], 0);
+            }
+        }
         for (i = r0; i < r1; i++)
             if (a->d_kind[i] == 1 && e.l2m.hash) chain_skipped_record(&e, i, a->d_off[i], a->d_len[i]);
-        free(put_off);
+        free(tlist); free(dlist);
         hs_launches += 1;
     }
     else {
