@@ -2003,6 +2003,7 @@ FLB_HDN void f_recmod(const struct ch_env *e, const struct ch_lane *ln, const st
 #define CH_MAX32(p, v)      atomicMax((unsigned int *) (p), (unsigned int) (v))
 #define CH_ADDF64(p, v)     atomicAdd((double *) (p), (double) (v))
 #define CH_ADD64(p, v)      atomicAdd((unsigned long long *) (p), (unsigned long long) (v))
+#define CH_MAX64(p, v)      atomicMax((unsigned long long *) (p), (unsigned long long) (v))
 /* gauge: the pair (record index + 1, value bits) of the LAST record of a label set wins, whatever order the
  * lanes arrive in -- cmt_gauge_set() overwrites in record order.  One 16-byte compare-and-swap (sm_90+). */
 struct __align__(16) ch_pair16 { unsigned long long a, b; };
@@ -2023,6 +2024,7 @@ static inline unsigned long long ch_cas64_host(unsigned long long *p, unsigned l
 #define CH_CAS64(p, c, v)   ch_cas64_host((unsigned long long *) (p), (c), (v))
 #define CH_MAX32(p, v)      do { if (*(p) < (v)) *(p) = (v); } while (0)
 #define CH_ADDF64(p, v)     (*(p) += (v))
+#define CH_MAX64(p, v)      do { if (*(p) < (v)) *(p) = (v); } while (0)
 static inline unsigned long long ch_add64_host(unsigned long long *p, unsigned long long v) { unsigned long long o = *p; *p = o + v; return o; }
 #define CH_ADD64(p, v)      ch_add64_host((unsigned long long *) (p), (v))
 #endif
@@ -2184,6 +2186,15 @@ FLB_HDN void f_l2m(const struct ch_env *e, const struct ch_lane *ln, const struc
         }
         CH_ATOMIC_ADD(&tb->bkt[(size_t) idx * (cf->n_buckets + 1) + cf->n_buckets], 1ull);
         CH_ADDF64(&tb->sum[idx], val);
+        if (tb->amax) {
+            union { double d; unsigned long long u; } cv;
+            const double av = val < 0 ? -val : val;
+            unsigned long long ai = av <= (double) L2M_EXACT_MAX ? (unsigned long long) av : L2M_NOT_EXACT;   /* NaN: not <= */
+            cv.d = val;
+            if ((double) ai != av || cv.u == 0x8000000000000000ull) ai = L2M_NOT_EXACT;
+            if (ai > tb->amax[idx]) CH_MAX64(&tb->amax[idx], ai);      /* (a plain read first: the hot sets' maximum is soon reached) */
+            if (tb->obs_slot) { tb->obs_slot[ridx] = idx + 1; tb->obs_val[ridx] = val; }
+        }
     }
     else if (cf->mode == L2M_GAUGE) {              /* bkt is [slot][2] here: last record index + 1, value bits */
         union { double d; unsigned long long u; } cv;

@@ -242,8 +242,18 @@ struct l2m_table {
      * pending_n[0] = listed, [1] = done. */
     uint32_t *pending;
     unsigned long long *pending_n;
+    /* histogram: the reference adds every observation to the set's sum in record order (cmt_metric_hist_sum_add()), which
+     * the atomic sum above matches only when every addition is exact.  amax[slot] = the largest |value| of the call's
+     * observations when all of them are integers of at most 2^53 (and none is -0.0), else L2M_NOT_EXACT; the host keeps the
+     * atomic sum where that proves it exact, and otherwise adds obs_val up in record order.  obs_slot[record] = slot + 1 of
+     * the record's observation (0: none), indexed by the call's record index. */
+    unsigned long long *amax;
+    uint32_t *obs_slot;
+    double *obs_val;
 };
 #define L2M_PENDING_CAP 65536u
+#define L2M_NOT_EXACT 0xffffffffffffffffull
+#define L2M_EXACT_MAX 9007199254740992ull      /* 2^53: every integer up to here is a double */
 
 struct chain_filter { uint32_t kind, cfg_off; };
 

@@ -119,6 +119,11 @@ struct l2m_set {
     double sum;
     uint64_t *buckets;       /* n_buckets + 1 */
     uint64_t call_last;      /* gauge: last record index + 1 seen for this set in the call being folded in */
+    /* histogram: a bound on |sum| while the sum is an integer reached by exact additions only (L2M_NOT_EXACT: no longer).
+     * While bound + count x max |value| of a call stays <= 2^53, any order of adding gives the record-order sum. */
+    uint64_t bound;
+    uint64_t call_n, call_amax;  /* histogram: observations of the call being folded in, and their amax */
+    double call_sum;             /* ... their atomic sum */
 };
 struct l2m_state {
     int mode, n_labels, n_buckets, discard;
@@ -195,6 +200,9 @@ struct flbgpu_chain {
     struct l2m_table l2m;                     /* device table (per-call delta) */
     size_t l2m_slots;
     uint64_t *h_hash, *h_chash, *h_cnt, *h_bkt; uint32_t *h_first; double *h_sum;    /* host mirror */
+    uint64_t *h_amax; int32_t *h_setof;       /* histogram: the slots' amax, and the set each slot of a call folds into */
+    uint32_t *h_obs_slot; double *h_obs_val; size_t cap_hobs;   /* histogram: the observations of a call, when one set needs them */
+    int l2m_record;                           /* histogram: the evaluation writes its observations (from the first call that needed them on) */
     /* device buffers, grown on demand */
     uint8_t *d_in;  size_t cap_in;
     uint8_t *d_out; size_t cap_out;
@@ -1532,6 +1540,11 @@ int flbgpu_chain_init(flbgpu_chain *c)
         }
         c->h_hash = malloc(n * 8); c->h_chash = malloc(n * 8); c->h_first = malloc(n * 4); c->h_cnt = malloc(n * 8); c->h_sum = malloc(n * 8);
         c->h_bkt = malloc(n * nbk * 8);
+        if (st->mode == L2M_HISTOGRAM) {
+            c->l2m.amax = bk_alloc(c->q, n * 8);
+            c->h_amax = malloc(n * 8); c->h_setof = malloc(n * sizeof(int32_t));
+            if (!c->l2m.amax || !c->h_amax || !c->h_setof) return -1;
+        }
         if (!c->l2m.hash || !c->l2m.chash || !c->l2m.first || !c->l2m.cnt || !c->l2m.sum || !c->l2m.bkt || !c->l2m.str) return -1;
     }
     if (bk_h2d(c->q, c->d_blob, c->blob.p, c->blob.n) || bk_sync(c->q)) return -1;
@@ -1562,7 +1575,9 @@ void flbgpu_chain_destroy(flbgpu_chain *c)
     bk_free(c->q, c->d_tl_bsum); free(c->h_tl_bsum);
     bk_free(c->q, c->d_esize); bk_free(c->q, c->d_ebsum); free(c->h_ebsum);
     bk_free(c->q, c->l2m.hash); bk_free(c->q, c->l2m.chash); bk_free(c->q, c->l2m.first); bk_free(c->q, c->l2m.cnt); bk_free(c->q, c->l2m.sum); bk_free(c->q, c->l2m.bkt); bk_free(c->q, c->l2m.str); bk_free(c->q, c->l2m.pending); bk_free(c->q, c->l2m.pending_n);
+    bk_free(c->q, c->l2m.amax); bk_free(c->q, c->l2m.obs_slot); bk_free(c->q, c->l2m.obs_val);
     free(c->h_hash); free(c->h_chash); free(c->h_first); free(c->h_cnt); free(c->h_sum); free(c->h_bkt);
+    free(c->h_amax); free(c->h_setof); free(c->h_obs_slot); free(c->h_obs_val);
     free(c->blob.p);
     if (c->ctx && c->ctx->last_q == c->q) c->ctx->last_q = NULL;
     bk_q_free(c->q);
@@ -1693,6 +1708,14 @@ static int ensure_rec_cap(flbgpu_chain *c, size_t need, size_t keep)
         bk_free(c->q, c->d_prep);
         c->d_prep = np_;
     }
+    if (c->l2m.amax) {                                 /* histogram observations, "none" for the new records */
+        uint32_t *ns_ = bk_alloc(c->q, nc * 4);
+        double *nv = bk_alloc(c->q, nc * 8);
+        if (!ns_ || !nv || bk_zero(c->q, ns_, nc * 4)) return -1;
+        if (keep && (bk_sync(c->q) || bk_d2d(c->q, ns_, c->l2m.obs_slot, keep * 4) || bk_d2d(c->q, nv, c->l2m.obs_val, keep * 8))) return -1;
+        bk_free(c->q, c->l2m.obs_slot); bk_free(c->q, c->l2m.obs_val);
+        c->l2m.obs_slot = ns_; c->l2m.obs_val = nv;
+    }
     if (keep) {
         if (bk_sync(c->q)) return -1;                 /* running kernels still read the old arrays */
         if (bk_d2d(c->q, o, c->d_off, keep * 4) || bk_d2d(c->q, l, c->d_len, keep * 4) || bk_d2d(c->q, z, c->d_size, keep * 4) ||
@@ -1763,6 +1786,7 @@ static void fill_args(flbgpu_chain *c, struct bk_chain_args *a, const uint8_t *d
     a->d_off = c->d_off; a->d_len = c->d_len; a->d_kind = c->d_kind; a->n_rec = n_rec;
     a->d_size = c->d_size; a->d_bsum = c->d_bsum; a->d_flags = c->d_flags;
     if (c->l2m_index >= 0 && ((c->active >> c->l2m_index) & 1)) a->l2m = c->l2m; else memset(&a->l2m, 0, sizeof(a->l2m));
+    if (!c->l2m_record) a->l2m.obs_slot = NULL, a->l2m.obs_val = NULL;
     a->active = c->active;
     a->scr_mul = c->scr_mul ? c->scr_mul : 4;
     a->defer_ok = (uint32_t) c->defer_ok;
@@ -1804,6 +1828,79 @@ static int l2m_clear(flbgpu_chain *c)
     if (bk_zero(c->q, c->l2m.hash, n * 8) || bk_zero(c->q, c->l2m.first, n * 4) || bk_zero(c->q, c->l2m.cnt, n * 8) ||
         bk_zero(c->q, c->l2m.sum, n * 8) || bk_zero(c->q, c->l2m.bkt, n * L2M_NBK(st) * 8)) return -1;
     if (c->l2m.pending_n && bk_zero(c->q, c->l2m.pending_n, 16)) return -1;
+    if (c->l2m.amax && bk_zero(c->q, c->l2m.amax, n * 8)) return -1;
+    if (c->l2m_record && c->l2m.obs_slot && bk_zero(c->q, c->l2m.obs_slot, c->cap_rec * 4)) return -1;
+    return 0;
+}
+
+/* histogram: 1 when the settled table holds a set whose sum has to be added up in record order (l2m_fold_sums) while this
+ * call's evaluation did not write its observations -- from now on it does, and the call evaluates again.  Conservative: any
+ * set that left the exact path, any observation that is not an exact integer, or all observations against the largest bound. */
+static int l2m_want_observations(flbgpu_chain *c)
+{
+    struct l2m_state *st;
+    size_t n = c->l2m_slots, i;
+    uint64_t maxb = 0, amax = 0, cnt = 0;
+    int need = 0, j;
+    if (c->l2m_record || !c->l2m.amax || c->l2m_index < 0 || !((c->active >> c->l2m_index) & 1)) return 0;
+    st = c->f[c->l2m_index]->l2m;
+    if (bk_d2h(c->q, c->h_hash, c->l2m.hash, n * 8) || bk_d2h(c->q, c->h_cnt, c->l2m.cnt, n * 8) ||
+        bk_d2h(c->q, c->h_amax, c->l2m.amax, n * 8) || bk_sync(c->q)) return -1;
+    for (j = 0; j < st->n_sets; j++) if (st->sets[j].bound > maxb) maxb = st->sets[j].bound;
+    for (i = 0; i < n; i++) {
+        if (!c->h_hash[i]) continue;
+        cnt += c->h_cnt[i];
+        if (c->h_amax[i] > amax) amax = c->h_amax[i];
+    }
+    if (cnt) need = maxb == L2M_NOT_EXACT || amax == L2M_NOT_EXACT || (amax && cnt > (L2M_EXACT_MAX - maxb) / amax);
+    if (need) c->l2m_record = 1;
+    return need;
+}
+
+/* the bound (struct l2m_set) a histogram sum starts from: |sum| when it is an integer of at most 2^53 other than -0.0 */
+static uint64_t l2m_sum_bound(double sum)
+{
+    const double a = sum < 0 ? -sum : sum;
+    uint64_t bits;
+    memcpy(&bits, &sum, 8);
+    if (!(a <= (double) L2M_EXACT_MAX) || (double) (uint64_t) a != a || bits == 0x8000000000000000ull) return L2M_NOT_EXACT;
+    return (uint64_t) a;
+}
+
+/* histogram: the sums of the sets the call observed.  A set keeps the atomic sum while it provably equals the record-order
+ * sum; otherwise its observations are added to its previous sum one by one, in record order, as cmt_metric_hist_sum_add()
+ * does (new = old + val). */
+static int l2m_fold_sums(flbgpu_chain *c, struct l2m_state *st, uint32_t n_rec)
+{
+    int i, any = 0;
+    uint32_t r;
+    for (i = 0; i < st->n_sets; i++) {
+        struct l2m_set *s = &st->sets[i];
+        if (!s->call_n) continue;
+        if (s->bound != L2M_NOT_EXACT && s->call_amax != L2M_NOT_EXACT &&
+            (s->call_amax == 0 || s->call_n <= (L2M_EXACT_MAX - s->bound) / s->call_amax)) {
+            s->sum += s->call_sum;
+            s->bound += s->call_n * s->call_amax;
+            s->call_n = 0;
+        }
+        else { s->bound = L2M_NOT_EXACT; any = 1; }
+    }
+    if (!any) return 0;
+    if (!c->l2m_record) { set_err("log_to_metrics: histogram observations were not recorded%s%s", NULL, NULL); return -1; }
+    if (c->cap_hobs < n_rec) {
+        free(c->h_obs_slot); free(c->h_obs_val);
+        c->cap_hobs = (size_t) n_rec + n_rec / 4 + 64;
+        c->h_obs_slot = malloc(c->cap_hobs * sizeof(uint32_t)); c->h_obs_val = malloc(c->cap_hobs * sizeof(double));
+        if (!c->h_obs_slot || !c->h_obs_val) { c->cap_hobs = 0; set_err("out of memory%s%s", NULL, NULL); return -1; }
+    }
+    if (n_rec && (bk_d2h(c->q, c->h_obs_slot, c->l2m.obs_slot, (size_t) n_rec * 4) ||
+                  bk_d2h(c->q, c->h_obs_val, c->l2m.obs_val, (size_t) n_rec * 8) || bk_sync(c->q))) return -1;
+    for (r = 0; r < n_rec; r++) {
+        struct l2m_set *s;
+        if (!c->h_obs_slot[r]) continue;
+        s = &st->sets[c->h_setof[c->h_obs_slot[r] - 1]];
+        if (s->call_n) s->sum += c->h_obs_val[r];
+    }
     return 0;
 }
 
@@ -1816,7 +1913,7 @@ static int cmp_first(const void *a, const void *b, void *arg)
 
 /* fold the settled per-call table into the filter's cumulative state, new label sets in
  * first-seen (record) order -- the order cmetrics appends them (cmt_map.c:209-243) */
-static int l2m_merge(flbgpu_chain *c)
+static int l2m_merge(flbgpu_chain *c, uint32_t n_rec)
 {
     struct l2m_state *st;
     size_t n = c->l2m_slots, nbk, i, m = 0;
@@ -1825,10 +1922,11 @@ static int l2m_merge(flbgpu_chain *c)
     st = c->f[c->l2m_index]->l2m;
     nbk = L2M_NBK(st);
     if (bk_d2h(c->q, c->h_hash, c->l2m.hash, n * 8) || bk_d2h(c->q, c->h_chash, c->l2m.chash, n * 8) || bk_d2h(c->q, c->h_first, c->l2m.first, n * 4) || bk_d2h(c->q, c->h_cnt, c->l2m.cnt, n * 8) ||
-        bk_d2h(c->q, c->h_sum, c->l2m.sum, n * 8) || bk_d2h(c->q, c->h_bkt, c->l2m.bkt, n * nbk * 8) || bk_sync(c->q)) return -1;
+        bk_d2h(c->q, c->h_sum, c->l2m.sum, n * 8) || bk_d2h(c->q, c->h_bkt, c->l2m.bkt, n * nbk * 8) ||
+        (c->l2m.amax && bk_d2h(c->q, c->h_amax, c->l2m.amax, n * 8)) || bk_sync(c->q)) return -1;
     order = malloc(sizeof(uint32_t) * (n ? n : 1));
     if (!order) { set_err("out of memory%s%s", NULL, NULL); return -1; }
-    for (i = 0; i < (size_t) st->n_sets; i++) st->sets[i].call_last = 0;
+    for (i = 0; i < (size_t) st->n_sets; i++) { st->sets[i].call_last = 0; st->sets[i].call_n = st->sets[i].call_amax = 0; st->sets[i].call_sum = 0; }
     for (i = 0; i < n; i++) if (c->h_hash[i]) order[m++] = (uint32_t) i;
     qsort_r(order, m, sizeof(uint32_t), cmp_first, c->h_first);
     for (i = 0; i < m; i++) {
@@ -1862,11 +1960,15 @@ static int l2m_merge(flbgpu_chain *c)
             if (c->h_bkt[slot * 2] > set->call_last) { set->call_last = c->h_bkt[slot * 2]; memcpy(&set->sum, &c->h_bkt[slot * 2 + 1], 8); }
             continue;
         }
-        set->sum += c->h_sum[slot];
         for (k = 0; k < nbk; k++) set->buckets[k] += c->h_bkt[slot * nbk + k];
+        if (st->mode != L2M_HISTOGRAM) continue;
+        c->h_setof[slot] = (int32_t) (set - st->sets);
+        set->call_n += c->h_cnt[slot];
+        set->call_sum += c->h_sum[slot];
+        if (c->h_amax[slot] > set->call_amax) set->call_amax = c->h_amax[slot];
     }
     free(order);
-    return 0;
+    return st->mode == L2M_HISTOGRAM ? l2m_fold_sums(c, st, n_rec) : 0;
 }
 
 
@@ -2138,7 +2240,9 @@ static int rtag_collect(flbgpu_chain *c, const struct bk_chain_args *a, uint32_t
  * verdict is (a chunk that does not decode to its end makes it NOTOUCH after the fact, rewrite_tag.c:500-546). */
 static int call_commit(flbgpu_chain *c, struct bk_chain_args *a, const uint8_t *d_in, size_t bytes, uint32_t n_rec, const uint32_t *flags)
 {
-    if (l2m_merge(c)) return -1;
+    const int again = l2m_want_observations(c);
+    if (again) return again;                         /* 1: evaluate the call again (its result is not committed), -1 */
+    if (l2m_merge(c, n_rec)) return -1;
     if (c->rtag_index < 0 || !((c->active >> c->rtag_index) & 1)) return 0;
     fill_args(c, a, d_in, bytes, n_rec);
     return rtag_collect(c, a, n_rec, (flags[c->rtag_index] & CHF_CAUSE) != 0);
@@ -2185,7 +2289,7 @@ static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_e
     uint32_t n_rec = 0, h_flags[FLBGPU_MAX_FILTERS + 1], nb;
     size_t off = 0, S = slice_bytes();
     uint64_t total;
-    int clean, pass;
+    int clean, pass, r;
     struct timespec t0;
 
     if (call_start(c, bytes, out_size, &t0) || !(d_in = place_input(c, h_in, d_in_ext, bytes)) ||
@@ -2224,7 +2328,12 @@ static int chain_run(flbgpu_chain *c, const uint8_t *h_in, const uint8_t *d_in_e
     }
     c->st.kernel_launches = bk_launch_count();
     c->st.phase_ms[0] = ms_since(&t0);
-    if (call_commit(c, &a, d_in, bytes, n_rec, h_flags)) return -1;
+    while ((r = call_commit(c, &a, d_in, bytes, n_rec, h_flags)) == 1) {      /* again, writing the metric observations */
+        fill_args(c, &a, d_in, bytes, n_rec);
+        if (bk_flags_clear(c->q, c->d_flags) || l2m_clear(c) || report_clear(c) || bk_chain_eval(c->q, &a, 0, n_rec)) return -1;
+        c->st.passes++;
+    }
+    if (r) return -1;
     if (a.assume == 0) return FLBGPU_FILTER_NOTOUCH;
 
     /* ---- output offsets ---- */
@@ -2413,7 +2522,11 @@ static int chain_run_stream(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, 
     }
     c->st.kernel_launches = bk_launch_count();
     if (so.dl_open) { so.dl_open = 0; if (bk_download_end(c->q)) goto fail; }
-    if (call_commit(c, &a, c->d_in, bytes, n_rec, h_flags)) goto fail;      /* every record of the call is still indexed */
+    switch (call_commit(c, &a, c->d_in, bytes, n_rec, h_flags)) {          /* every record of the call is still indexed */
+    case 0: break;
+    case 1: stream_drop(c, &so); return 1;          /* the metric observations are wanted: the classic path writes them */
+    default: goto fail;
+    }
     bk_records_out(c->q, &c->st.records_out);
     c->st.bytes_out = so.placed;
     *out_size = (size_t) so.placed;
@@ -2493,7 +2606,11 @@ static int chain_run_small(flbgpu_chain *c, const uint8_t *h_in, size_t bytes, v
         c->small_cap_out = (size_t) res.total + (size_t) res.total / 4 + 4096;
         return 1;
     }
-    if (call_commit(c, &a, c->d_in, bytes, res.n_valid, res.flags)) return -1;
+    switch (call_commit(c, &a, c->d_in, bytes, res.n_valid, res.flags)) {
+    case 0: break;
+    case 1: return 1;                                /* the metric observations are wanted: the general paths write them */
+    default: return -1;
+    }
     c->st.records_out = res.n_out;
     c->st.bytes_out = res.total;
     *out_size = (size_t) res.total;
@@ -2669,7 +2786,7 @@ int flbgpu_l2m_put(flbgpu_filter *f, uint64_t hash, uint64_t count, double sum, 
     }
     set = &st->sets[st->n_sets++];
     memset(set, 0, sizeof(*set));
-    set->hash = hash; set->count = count; set->sum = sum;
+    set->hash = hash; set->count = count; set->sum = sum; set->bound = l2m_sum_bound(sum);
     set->labels = malloc(lb); memcpy(set->labels, labels, lb);
     set->buckets = calloc(st->n_buckets + 1, sizeof(uint64_t));
     if (buckets) memcpy(set->buckets, buckets, sizeof(uint64_t) * (st->n_buckets + 1));
@@ -3119,6 +3236,7 @@ int flbgpu_l2m_allreduce(flbgpu_filter *f)
         else {
             memcpy(merged[j].buckets, row + 1, ((size_t) st->n_buckets + 1) * 8);
             merged[j].sum = h_sum[j];
+            merged[j].bound = l2m_sum_bound(merged[j].sum);
         }
     }
     for (i = 0; i < st->n_sets; i++) { free(st->sets[i].labels); free(st->sets[i].buckets); }

@@ -207,8 +207,19 @@ static uint32_t hs_raw_lo(const struct bk_chain_args *a, uint32_t i)
 int bk_flags_clear(bk_q *q, uint32_t *d_flags) { memset(d_flags, 0, sizeof(uint32_t) * (FLBGPU_MAX_FILTERS + 1)); q->records_out = 0; return 0; }
 int bk_flags_fetch(bk_q *, const uint32_t *d_flags, uint32_t *h_flags) { memcpy(h_flags, d_flags, sizeof(uint32_t) * (FLBGPU_MAX_FILTERS + 1)); return 0; }
 
+/* FLBGPU_SIM_ORDER=reverse: every record loop of an evaluation runs from its last entry to its first.  The kernels give no
+ * order among a launch's records; this is the emulation's other extreme, for results that must not depend on it. */
+static int hs_reverse(void)
+{
+    const char *e = getenv("FLBGPU_SIM_ORDER");
+    return e && !strcmp(e, "reverse");
+}
+/* entry t of a loop over n entries, in the emulation's order */
+static inline uint32_t hs_at(uint32_t t, uint32_t n, int rev) { return rev ? n - 1 - t : t; }
+
 int bk_chain_eval(bk_q *, const struct bk_chain_args *a, uint32_t r0, uint32_t r1)
 {
+    const int rev = hs_reverse();
     struct ch_env e;
     uint32_t i;
     uint32_t *bm = 0;
@@ -235,8 +246,10 @@ int bk_chain_eval(bk_q *, const struct bk_chain_args *a, uint32_t r0, uint32_t r
         const int defer_first = getenv("FLBGPU_SIM_DEFER_FIRST") && getenv("FLBGPU_SIM_DEFER_FIRST")[0] == '1';
         uint32_t *tlist = (uint32_t *) malloc(sizeof(uint32_t) * (r1 - r0 + 1)), *dlist = (uint32_t *) malloc(sizeof(uint32_t) * (r1 - r0 + 1));
         uint32_t tn = 0, dn = 0, t;
-        for (i = r0; i < r1; i++) {
+        /* (the lists fill in the head's order: under FLBGPU_SIM_ORDER=reverse the tail and the put-off records run backwards too) */
+        for (t = 0; t < r1 - r0; t++) {
             uint32_t sz = 0;
+            i = r0 + hs_at(t, r1 - r0, rev);
             if (a->d_kind[i] == 0) ln.raw_lo = hs_raw_lo(a, i), sz = chain_record<false, CH_PH_HEAD>(&e, &ln, i, a->d_off[i], a->d_len[i], 0);
             if (sz == CH_DEFER) { dlist[dn++] = i; sz = 0; }
             if (sz) tlist[tn++] = i;
@@ -253,8 +266,8 @@ int bk_chain_eval(bk_q *, const struct bk_chain_args *a, uint32_t r0, uint32_t r
                 a->d_size[i] = chain_record<false>(&e, &plain, i, a->d_off[i], a->d_len[i], 0);
             }
         }
-        for (i = r0; i < r1; i++)
-            if (a->d_kind[i] == 1 && e.l2m.hash) chain_skipped_record(&e, i, a->d_off[i], a->d_len[i]);
+        for (t = 0; t < r1 - r0; t++)
+            if (i = r0 + hs_at(t, r1 - r0, rev), a->d_kind[i] == 1 && e.l2m.hash) chain_skipped_record(&e, i, a->d_off[i], a->d_len[i]);
         free(tlist); free(dlist);
         hs_launches += 1;
     }
@@ -262,19 +275,22 @@ int bk_chain_eval(bk_q *, const struct bk_chain_args *a, uint32_t r0, uint32_t r
         uint8_t *put_off = (uint8_t *) calloc(r1 - r0 + 1, 1);
         struct ch_lane plain;
         memset(&plain, 0, sizeof(plain));
-        for (i = r0; i < r1; i++) {
+        uint32_t t;
+        for (t = 0; t < r1 - r0; t++) {
             uint32_t sz = 0;
+            i = r0 + hs_at(t, r1 - r0, rev);
             if (a->d_kind[i] == 0) ln.raw_lo = hs_raw_lo(a, i), sz = chain_record<false>(&e, &ln, i, a->d_off[i], a->d_len[i], 0);
             else if (a->d_kind[i] == 1 && e.l2m.hash) chain_skipped_record(&e, i, a->d_off[i], a->d_len[i]);
             if (sz == CH_DEFER) { put_off[i - r0] = 1; sz = 0; }
             a->d_size[i] = sz;
         }
-        for (i = r0; i < r1; i++)
-            if (put_off[i - r0]) { plain.raw_lo = hs_raw_lo(a, i); a->d_size[i] = chain_record<false>(&e, &plain, i, a->d_off[i], a->d_len[i], 0); }
+        for (t = 0; t < r1 - r0; t++)
+            if (i = r0 + hs_at(t, r1 - r0, rev), put_off[i - r0]) { plain.raw_lo = hs_raw_lo(a, i); a->d_size[i] = chain_record<false>(&e, &plain, i, a->d_off[i], a->d_len[i], 0); }
         free(put_off);
     }
     free(bm);
-    if (e.l2m.hash && e.l2m.pending) {             /* k_l2m_fixup: the records whose value text converts nothing */
+    if (e.l2m.hash && e.l2m.pending) {             /* k_l2m_fixup: the records whose value text converts nothing, in the list's
+                                                    * order (backwards under FLBGPU_SIM_ORDER=reverse, as the evaluation filled it) */
         unsigned long long n = e.l2m.pending_n[0], d = e.l2m.pending_n[1], t;
         if (n > e.l2m.pending_cap) n = e.l2m.pending_cap;
         for (t = d; t < n; t++) l2m_fixup_record(&e, e.l2m.pending[t], a->d_off, a->d_len, a->d_kind);
